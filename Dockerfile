@@ -1,4 +1,4 @@
-# Operator + runtime image for one 8xB200 box (counterpart of the reference's Dockerfile + build/base/*.Dockerfile:
+# Operator + runtime image for one 8xH100 box (counterpart of the reference's Dockerfile + build/base/*.Dockerfile:
 # there the operator is a distroless Go binary and MPI/sshd live in separate user images; here one image carries the
 # daemon, the native launcher, the collective runtime and the example workloads).
 #   docker build -t mpi-operator-b200 . && docker run --gpus all --ipc=host --network=host mpi-operator-b200

@@ -1,9 +1,9 @@
-# b200mpi native build (sm_100a only). `make` builds everything in-tree; the
-# built artefacts are git-ignored but travel to the GPU box with gpurun.
+# b200mpi native build (sm_90a only). `make` builds everything in-tree; the
+# built artefacts are git-ignored.
 comma     := ,
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := -std=c++17 -O3 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Icsrc/include
 CXXFLAGS  := -std=c++17 -O2 -fPIC -Wall -Icsrc/include
 LIBDIR    := mpi_operator_b200/lib
@@ -25,7 +25,7 @@ $(LIBDIR)/libb200mpi_nccl.so: csrc/nccl_shim/nccl_shim.cu $(RUNTIME_SRCS) $(RUNT
 	@mkdir -p $(LIBDIR)
 	$(NVCC) $(NVFLAGS) -shared -x cu csrc/nccl_shim/nccl_shim.cu $(RUNTIME_SRCS) -o $@ -lrt -lpthread -ldl
 
-# tcgen05/TMA GEMM with fused BN statistics: a library of its own so that the experimental kernel cannot affect
+# wgmma/TMA GEMM with fused BN statistics: a library of its own so that the experimental kernel cannot affect
 # the validated runtime library
 $(LIBDIR)/libb200mpi_gemm.so: csrc/kernels/gemm_bnstats.cu csrc/kernels/gemm_bnstats_logic.h csrc/include/b200mpi.h
 	@mkdir -p $(LIBDIR)
@@ -129,18 +129,18 @@ test_p2p_protocol: $(LIBDIR)/libb200mpi.so
 	$(NVCC) -std=c++17 -O1 $(ARCH) -Icsrc/include -Xcudafe --diag_suppress=20011,--diag_suppress=20014 -x cu csrc/tests/p2p_protocol_test.cu -o build/san/p2p_protocol_test -L$(LIBDIR) -lb200mpi -Xlinker -rpath,$(abspath $(LIBDIR)) -lrt -lpthread
 	build/san/p2p_protocol_test
 
-# host model of the tcgen05 GEMM's three-role pipeline (shares gemm_bnstats_logic.h with the kernel)
+# host model of the wgmma GEMM's producer / consumer pipeline (shares gemm_bnstats_logic.h with the kernel)
 test_gemm_model:
 	@mkdir -p build/san
 	$(CXX) -std=c++17 -O2 -Wall -o build/san/gemm_pipeline_model csrc/tests/gemm_pipeline_model.cc -lpthread
 	build/san/gemm_pipeline_model
 
-# hand-packed tcgen05 descriptors vs CuTe's (headers vendored with flashinfer in this image; pass CUTLASS_INC=... elsewhere)
+# hand-packed wgmma descriptor vs CuTe's (CUTLASS headers as shipped with the flashinfer wheel; pass CUTLASS_INC=... elsewhere)
 CUTLASS_INC ?= $(shell python -c "import importlib.util,os;s=importlib.util.find_spec('flashinfer');print(os.path.join(os.path.dirname(s.origin),'data','cutlass','include'))" 2>/dev/null)
-test_umma_desc:
+test_gmma_desc:
 	@mkdir -p build/san
-	$(NVCC) -std=c++17 -O1 $(ARCH) --expt-relaxed-constexpr -Icsrc/include -I$(CUTLASS_INC) -x cu csrc/tests/umma_desc_test.cu -o build/san/umma_desc_test
-	build/san/umma_desc_test 2>/dev/null
+	$(NVCC) -std=c++17 -O1 $(ARCH) --expt-relaxed-constexpr -Icsrc/include -I$(CUTLASS_INC) -x cu csrc/tests/gmma_desc_test.cu -o build/san/gmma_desc_test
+	build/san/gmma_desc_test 2>/dev/null
 
 asan:
 	$(call san_build,asan,-fsanitize=address$(comma)undefined -fno-sanitize-recover=undefined)
@@ -155,10 +155,10 @@ tsan:
 	build/san/tsan/mpirun -n 2 build/san/tsan/pi
 	TSAN_OPTIONS=halt_on_error=1 build/san/tsan/mpirun -n 4 build/san/tsan/hvd_core_test
 	# device protocols executed by host threads (same templates / shared logic as the kernels) under ThreadSanitizer:
-	# every shared-memory, TMEM, mailbox and flag access must be ordered by the barriers the kernels use
+	# every shared-memory, mailbox and flag access must be ordered by the barriers the kernels use
 	$(SAN_CXX) -std=c++17 -O1 -g -fsanitize=thread -o build/san/tsan/gemm_pipeline_model csrc/tests/gemm_pipeline_model.cc -lpthread
 	TSAN_OPTIONS=halt_on_error=1 build/san/tsan/gemm_pipeline_model
 	$(NVCC) -ccbin $(SAN_CXX) -std=c++17 -O1 -g $(ARCH) -Icsrc/include -Xcudafe --diag_suppress=20011,--diag_suppress=20014 -Xcompiler -fsanitize=thread -x cu csrc/tests/p2p_protocol_test.cu -o build/san/tsan/p2p_protocol_test -L$(LIBDIR) -lb200mpi -Xlinker -rpath,$(abspath $(LIBDIR)) -lrt -lpthread -ltsan
 	TSAN_OPTIONS=halt_on_error=1 build/san/tsan/p2p_protocol_test
 
-.PHONY: all native sass clean test test_gpu test_e2e generate verify-generate lint sanitize asan tsan test_comm_host test_umma_desc test_p2p_protocol test_gemm_model test_mpi_p2p test_hvd_core
+.PHONY: all native sass clean test test_gpu test_e2e generate verify-generate lint sanitize asan tsan test_comm_host test_gmma_desc test_p2p_protocol test_gemm_model test_mpi_p2p test_hvd_core

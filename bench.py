@@ -10,7 +10,7 @@ tensorflow-benchmarks.yaml: --model=resnet101 --batch_size=64
       --master-port 29511 bench.py --gpus 8 --steps 20 --warmup 5
 
 --impl ours       (default) b200mpi: symmetric-window gradients, fused
-                  allreduce+SGD sm_100a kernels, whole step in a CUDA graph
+                  allreduce+SGD sm_90a kernels, whole step in a CUDA graph
 --impl nccl       same engine (fused BN kernels, CUDA graph), gradient allreduce via stock NCCL
                   (torch.distributed) + unfused optimizer: isolates what the collective runtime buys
 --impl torchddp   STOCK: torchvision's resnet101 + torch DDP + torch.optim.SGD, eager, bf16 autocast;
@@ -18,7 +18,9 @@ tensorflow-benchmarks.yaml: --model=resnet101 --batch_size=64
 --impl reference  the unmodified reference from baseline/_ref (a Go Kubernetes
                   operator: cannot run here -> prints {"unavailable": ...})
 
-Prints ONE JSON line on rank 0 (contract in the task description). After its own measurement `--impl ours` also runs
+Prints ONE JSON line on rank 0. --dump-outputs DIR also writes what the last step of the second timed phase (the
+end-to-end loop, which runs after the device-timed loop) computed: loss.npy, and params_sample.npy, a fixed, seeded sample
+of the fp32 parameters after that step, so that two builds can be compared on identical, seeded inputs. After its own measurement `--impl ours` also runs
 the two same-box baselines as child processes (one per rank, own rendezvous port, own timeout; a failing or hanging
 child cannot break the main line) and reports them under "same_box" with the ratios: the reference itself cannot run on
 this box (see reference_arm), so these are the only same-hardware, same-dtype comparators.
@@ -44,7 +46,7 @@ def reference_arm(args) -> int:
     ref = os.path.join(ROOT, "baseline", "_ref")
     why = ("reference is a Go Kubernetes operator (no Python package at /root/reference root; pip install fails: "
            "neither setup.py nor pyproject.toml) and its workload stack (Open MPI + Horovod + TensorFlow 1.14/2.3 "
-           "CUDA 10.1 images) is not installable offline nor runnable on sm_100")
+           "CUDA 10.1 images) is not installable offline nor runnable on sm_90")
     if os.path.isdir(ref) and os.listdir(ref):
         why = "baseline/_ref holds only the reference's generated Python SDK models (no training path, no operator): " + why
     print(json.dumps({"impl": "reference", "unavailable": why}))
@@ -52,7 +54,7 @@ def reference_arm(args) -> int:
 
 
 class ClockSampler:
-    """nvidia-smi clock/throttle sampling DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock/throttle sampling DURING the timed region."""
 
     def __init__(self, gpu_index: int):
         self.rows = []
@@ -111,7 +113,7 @@ def _clean_child_env(port_shift: int, job_suffix: str, extra: dict) -> dict:
     return env
 
 
-def _run_child(args, impl: str, env: dict, timeout: int):
+def _run_child(args, impl: str, env: dict, timeout: int, dump: str | None = None):
     """One measurement in a child process (this rank's GPU). Returns (rc, parsed JSON line or None, stderr tail)."""
     cmd = [sys.executable, os.path.abspath(__file__), "--impl", impl, "--child", "--gpus", str(args.gpus), "--steps", str(args.steps),
            "--warmup", str(args.warmup), "--model", args.model, "--batch-size", str(args.batch_size), "--dtype", args.dtype,
@@ -124,6 +126,8 @@ def _run_child(args, impl: str, env: dict, timeout: int):
         cmd += ["--algo", args.algo]
     if args.bucket_mb:
         cmd += ["--bucket-mb", str(args.bucket_mb)]
+    if dump:
+        cmd += ["--dump-outputs", dump]
     try:
         p = subprocess.Popen(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, start_new_session=True)
         try:
@@ -196,7 +200,7 @@ def supervise(args) -> int:
         _gemm.lib()
     except Exception as e:  # pragma: no cover  (a missing library fails loudly in the children)
         print(f"[bench supervisor] could not map the runtime libraries: {e}", file=sys.stderr)
-    result, used, notes, tried = None, None, [], {}
+    result, used, notes, tried, dumps = None, None, [], {}, {}
     k = 0
     for stage in stages(world):
         good = []
@@ -210,7 +214,8 @@ def supervise(args) -> int:
                 if not room:
                     notes.append(f"{name}: not tried (time budget)")
                     continue
-            rc, d, err = _run_child(args, "ours", _clean_child_env(17 * k, f"ours-{name}", extra), args.attempt_timeout)
+            dumps[name] = os.path.join(workdir, f"outputs-{name}") if args.dump_outputs else None
+            rc, d, err = _run_child(args, "ours", _clean_child_env(17 * k, f"ours-{name}", extra), args.attempt_timeout, dumps[name])
             ok_local = (rc == 0) and (rank != 0 or (d is not None and d.get("value")))
             ok = _agree(workdir, f"attempt{k}", rank, world, ok_local, args.attempt_timeout + 60) if world > 1 else ok_local
             if ok:
@@ -267,6 +272,11 @@ def supervise(args) -> int:
                 "what": "same box, same dtype, same batch, run right after the main measurement: nccl_same_engine = this "
                         "repo's trainer (fused BN kernels, CUDA graph) with the gradient allreduce on stock NCCL + unfused "
                         "SGD; torchddp_stock = torchvision resnet101 + torch DDP + torch.optim.SGD, eager, no repo code"}
+    if rank == 0 and args.dump_outputs:   # the outputs of the configuration the line reports
+        import shutil
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for f in os.listdir(dumps[used]):
+            shutil.copy(os.path.join(dumps[used], f), os.path.join(args.dump_outputs, f))
     if rank == 0:
         result.setdefault("config", {})["bench_configuration"] = used
         if len(tried) > 1:
@@ -283,6 +293,23 @@ def supervise(args) -> int:
         time.sleep(2.0 if world > 1 else 0.0)
         shutil.rmtree(workdir, ignore_errors=True)
     return 0
+
+
+DUMP_PARAM_SAMPLE = 1 << 22   # 16 MiB of fp32 parameters
+
+
+def dump_outputs(dirname: str, loss: float, params) -> None:
+    """What a caller of the timed path holds after its last step: the loss, and the fp32 (master) parameters in
+    module.parameters() order, flattened - as a fixed, seeded sample of DUMP_PARAM_SAMPLE elements when larger."""
+    import numpy as np
+    import torch
+    flat = torch.cat([p.detach().float().reshape(-1) for p in params]).cpu().numpy()
+    if flat.size > DUMP_PARAM_SAMPLE:
+        idx = np.sort(np.random.default_rng(0).choice(flat.size, DUMP_PARAM_SAMPLE, replace=False))
+        flat = flat[idx]
+    os.makedirs(dirname, exist_ok=True)
+    np.save(os.path.join(dirname, "loss.npy"), np.array([loss], dtype=np.float32))
+    np.save(os.path.join(dirname, "params_sample.npy"), flat.astype(np.float32))
 
 
 def main() -> int:
@@ -305,7 +332,11 @@ def main() -> int:
     ap.add_argument("--budget", type=int, default=int(os.environ.get("B200MPI_BENCH_BUDGET_S", 780)),
                     help="seconds the whole invocation may take; the same-box arms are skipped or shortened to stay inside it")
     ap.add_argument("--child", action="store_true", help="(internal) run the measurement in this process")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last end-to-end timed step (loss, sampled parameters) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return reference_arm(args)
     if args.warmup < 3:
@@ -414,7 +445,7 @@ def main() -> int:
             return trainer.step(host_x[i % nb], host_y[i % nb])
         launches_per_step = lambda: trainer.launches_per_step  # noqa: E731  (collective + fused BN / GEMM kernels of one step)
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -487,6 +518,13 @@ def main() -> int:
         print(f"[bench rank {rank}] self-check FAILED: {'; '.join(problems)}", file=sys.stderr, flush=True)
         return 7
 
+    if args.dump_outputs and rank == 0:
+        if args.impl == "torchddp":
+            params = [p.detach() for p in m.parameters()]
+        else:
+            params = list(trainer.state.master_state().values())
+        dump_outputs(args.dump_outputs, last_loss, params)
+
     import struct
     got = comm.host_allgather(struct.pack("dd", ms_dev, ms_e2e)) if world > 1 else [struct.pack("dd", ms_dev, ms_e2e)]
     ms_dev_max = max(struct.unpack("dd", g)[0] for g in got)
@@ -507,7 +545,7 @@ def main() -> int:
                            " (bf16 weight shadow refreshed by the fused SGD kernel)"
                            if args.impl != "torchddp" and getattr(trainer, "bf16_params", False) else ""),
                        "l2": "256 MiB buffer rewritten between timed steps (inside the timed region, device-timed and e2e "
-                             "phases alike); per-step activations also exceed the 126 MB L2",
+                             "phases alike); per-step activations also exceed the 50 MB L2",
                        "self_check": "finite loss; parameters bit-identical on all ranks; bf16 shadow == bf16(master)",
                        "baseline": "154.2 img/s/GPU x n_gpus (reference README.md:209, GPU unstated)",
                        "cuda_graph": (not args.no_graph) and args.impl != "torchddp",

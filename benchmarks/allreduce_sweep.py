@@ -2,8 +2,8 @@
 size for every b200mpi algorithm and for stock NCCL (torch.distributed), device
 timed with CUDA events, max over ranks.  Run one process per GPU, e.g.
   python tests/mp_launch.py -n 8 benchmarks/allreduce_sweep.py --out profiles/allreduce_sweep_n8.json
-busbw = algbw * 2(N-1)/N, reported against 900 GB/s per direction (nominal) and
-the measured 770 GB/s peer-copy figure (B200_PROFILING.md)."""
+busbw = algbw * 2(N-1)/N, reported against the H100 NVLink data-sheet rate
+(mpi_operator_b200.utils.roofline.LINK_GBS, 450 GB/s per direction)."""
 import argparse
 import json
 import os
@@ -15,6 +15,7 @@ import torch.distributed as dist
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from mpi_operator_b200.launch.env import rank_info_from_env  # noqa: E402
 from mpi_operator_b200.runtime.comm import Communicator  # noqa: E402
+from mpi_operator_b200.utils.roofline import LINK_GBS  # noqa: E402
 
 
 def time_op(fn, iters, warmup, comm, flush=None, inner=1):
@@ -126,7 +127,7 @@ def main():
                 algbw = size / (med_max * 1e-3) / 1e9
                 rows.append({"dtype": dname, "bytes": size, "algo": name, "ms_median_max_over_ranks": med_max,
                              "ms_best_max_over_ranks": best_max, "algbw_gbs": algbw, "busbw_gbs": algbw * factor,
-                             "busbw_frac_of_900": algbw * factor / 900.0, "busbw_frac_of_770_measured": algbw * factor / 770.0})
+                             "busbw_frac_of_link": algbw * factor / LINK_GBS})
                 if R == 0:
                     print(f"{dname:9s} {size:>11d} B {name:15s} {med_max * 1e3:10.1f} us  algbw {algbw:8.2f} GB/s  busbw {algbw * factor:8.2f} GB/s", flush=True)
             size *= 4 if size < (1 << 20) else 2

@@ -21,6 +21,9 @@ import sys
 import torch
 import torch.distributed as dist
 
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from mpi_operator_b200.utils.roofline import LINK_GBS  # noqa: E402
+
 
 def timed(fn, iters, warmup, inner):
     for _ in range(warmup):
@@ -101,7 +104,7 @@ def main():
                 algbw = nbytes / (med * 1e-3) / 1e9
                 rows.append({"impl": a.tag, "op": op, "dtype": dname, "bytes": nbytes, "us_median_max_over_ranks": med * 1e3,
                              "us_best_max_over_ranks": best * 1e3, "algbw_gbs": algbw, "busbw_gbs": algbw * factor,
-                             "busbw_frac_of_900": algbw * factor / 900.0, "graph_replay": graphed})
+                             "busbw_frac_of_link": algbw * factor / LINK_GBS, "graph_replay": graphed})
                 if rank == 0:
                     print(f"{a.tag:5s} {op:14s} {dname:9s} {nbytes:>11d} B {med * 1e3:10.1f} us  busbw {algbw * factor:8.2f} GB/s", flush=True)
                 del full, part

@@ -4,6 +4,10 @@ Usage: python benchmarks/roofline_per_op.py profiles/r2 --out profiles"""
 import argparse
 import json
 import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from mpi_operator_b200.utils.roofline import LINK_GBS  # noqa: E402
 
 
 def load(path):
@@ -18,11 +22,6 @@ def main():
     ap.add_argument("root")
     ap.add_argument("--out", default="profiles")
     a = ap.parse_args()
-    notes = {8: "measured with the final kernels of round 2 (TMA staging copies, registered paths)",
-             4: "measured BEFORE the copy stages of the pipelined kernel were fixed (pre-TMA): allreduce / broadcast / reduce_scatter rows >= 8 MiB "
-                "are the slow first version; see the probe logs in profiles/r2/n4 for the fixed kernel (587 GB/s busbw at 256 MiB)",
-             2: "measured with the FIRST version of the pipelined kernel and before cudaIpc registration existed: every row >= 8 MiB is stale "
-                "(the registered zero-copy path now serves those sizes at 2 GPUs; not re-measured, the GPU budget of the round was spent)"}
     per_op = {}
     for n in (8, 4, 2):
         nc, sh = load(f"{a.root}/n{n}/sweep_nccl_n{n}.json"), load(f"{a.root}/n{n}/sweep_shim_n{n}.json")
@@ -39,11 +38,11 @@ def main():
                "Same script (`benchmarks/collective_sweep.py`: torch.distributed on plain `torch.empty` tensors), same launcher, same box;",
                "CUDA events around CUDA-graph replays, median, max over ranks. busbw = algbw x " +
                {"allreduce": "2(N-1)/N", "allgather": "(N-1)/N", "reduce_scatter": "(N-1)/N", "broadcast": "1"}[op] +
-               "; the roofline is 900 GB/s per direction per GPU (NVLink 5), measured peer copy 770 GB/s.", ""]
+               f"; the roofline is {LINK_GBS:.0f} GB/s per direction per GPU (H100 SXM data sheet, NVLink 4).", ""]
         for n in sorted(by_n, reverse=True):
-            out += [f"## {n} GPUs - {notes[n]}", ""]
+            out += [f"## {n} GPUs", ""]
             for dt in sorted(by_n[n]):
-                out += [f"### {dt}", "", "| bytes | shim us | shim busbw GB/s | busbw / 900 | NCCL us | NCCL busbw GB/s | shim / NCCL |", "|---|---|---|---|---|---|---|"]
+                out += [f"### {dt}", "", f"| bytes | shim us | shim busbw GB/s | busbw / {LINK_GBS:.0f} | NCCL us | NCCL busbw GB/s | shim / NCCL |", "|---|---|---|---|---|---|---|"]
                 worst = None
                 for b in sorted(by_n[n][dt]):
                     v = by_n[n][dt][b]
@@ -52,7 +51,7 @@ def main():
                         continue
                     ratio = c["us_median_max_over_ranks"] / s["us_median_max_over_ranks"]
                     worst = ratio if worst is None else min(worst, ratio)
-                    out.append(f"| {b} | {s['us_median_max_over_ranks']:.1f} | {s['busbw_gbs']:.1f} | {s['busbw_frac_of_900']:.3f} | "
+                    out.append(f"| {b} | {s['us_median_max_over_ranks']:.1f} | {s['busbw_gbs']:.1f} | {s['busbw_gbs'] / LINK_GBS:.3f} | "
                                f"{c['us_median_max_over_ranks']:.1f} | {c['busbw_gbs']:.1f} | {ratio:.2f}x |")
                 out += ["", f"worst ratio: {worst:.2f}x" if worst else "", ""]
         if op == "allreduce":

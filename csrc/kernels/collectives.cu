@@ -1,4 +1,4 @@
-// b200mpi collective kernels for sm_100a: NVSwitch peer-memory allreduce
+// b200mpi collective kernels for sm_90a: NVSwitch peer-memory allreduce
 // (push one-shot, pull/push two-shot, NVLS multimem), fused allreduce+SGD,
 // allgather, broadcast, reduce-scatter, reduce, all-to-all, barrier.
 //
@@ -190,7 +190,7 @@ k_allreduce_twoshot(const __grid_constant__ KArgs a0, const KArgs* __restrict__ 
 //                   role 2  wait IN; (non-root) slot -> user buffer              -> RED (all ranks)
 //
 // so while chunk k is on NVLink, chunk k+1 is being copied in and chunk k-1 copied out: the local HBM copies that
-// serialised the old staged kernels (three phases, two full barriers: 370 GB/s at 8 GPUs for allreduce) disappear behind
+// serialised the old staged kernels (three phases, two full barriers) disappear behind
 // the link time. A slot is refilled for chunk k+depth only after every rank that reads or writes it for chunk k has
 // said so (local counter for allreduce, RED flags otherwise). Flags only grow (per-role, per-lane counters persist in
 // the epoch array and advance identically for all three roles), so the kernel is CUDA-graph capturable like the others.
@@ -198,8 +198,7 @@ k_allreduce_twoshot(const __grid_constant__ KArgs a0, const KArgs* __restrict__ 
 // ---- TMA bulk copies for the pipeline's local staging copies ------------------------------------------------------
 // One elected thread moves a chunk global -> shared -> global with cp.async.bulk (SASS UBLKCP): a ring of kBulkNB
 // buffers, up to kBulkNB/2 loads and kBulkNB/2 stores in flight (96 KB each way per CTA) with no registers and no
-// warps tied up - a 512-thread CTA doing 16-byte loads/stores topped out at ~26 GB/s (timeline: 40 us per MiB), which
-// made the copy stages as slow as the NVLS stage they are supposed to hide behind.
+// warps tied up - a 512-thread CTA doing 16-byte loads/stores was slow enough to make the copy stages as slow as the NVLS stage they are supposed to hide behind.
 constexpr int kBulkNB = 8;
 constexpr uint32_t kBulkBytes = 24 * 1024;
 constexpr size_t kPipeSmemBytes = (size_t)kBulkNB * kBulkBytes + 128;   // + mbarriers
@@ -253,7 +252,7 @@ __device__ __forceinline__ void bulk_copy_drain() {
 // copy `len` vectors user -> staging (plain stores into local HBM), 8 loads in flight per thread.
 // The aligned, full-vector case is a separate loop on purpose: user_load()'s byte-wise tail takes the address of its
 // result, which parks the vector in local memory and makes every load wait for the previous one (measured with the
-// in-kernel timeline: 74 us per MiB per CTA = 14 GB/s, the bottleneck of the whole pipeline).
+// in-kernel timeline: the bottleneck of the whole pipeline).
 __device__ __forceinline__ void pipe_copy_in(char* dst, const char* ubase, size_t uvec0, size_t unbytes, bool ualigned, size_t len) {
   constexpr int U = 4;   // 32 KB in flight per CTA; 8 made the NVLS variants spill (128-register budget of 512-thread CTAs)
   if (ualigned && (uvec0 + len) * 16 <= unbytes) {
@@ -446,8 +445,7 @@ k_pipe(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu) {
       } else if (OP == PIPE_ALLGATHER || (OP == PIPE_BROADCAST && rank == a.root)) {
         // push: user chunk -> the same staging offset on every rank; allgather also writes its own output block directly
         const size_t dst = (slot + (OP == PIPE_ALLGATHER ? (size_t)rank * Cv : 0)) * 16;
-        // the root of a broadcast is the only rank that pushes: twice the loads in flight per CTA (8-GPU sweep of round 2:
-        // 388 GB/s with 4, against NCCL's 656)
+        // the root of a broadcast is the only rank that pushes: twice the loads in flight per CTA
         constexpr int U = OP == PIPE_BROADCAST ? 8 : 4;
         const bool fast_in = a.in_aligned && (v0 + len) * 16 <= a.nbytes;
         const bool fast_out = a.out_aligned && (v0 + len) * 16 <= a.nbytes;
@@ -640,8 +638,7 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
   const float wd = a.hyper ? __ldg(a.hyper + 2) : a.wd;
 
   // U vectors per thread per trip: U NVLink reduce-loads (or U x world peer loads) are issued before any
-  // is consumed — with one vector per trip the NVLS variant was latency-bound (~45 GB/s per rank, 1.2 ms
-  // exposed per step at 8 GPUs).
+  // is consumed — with one vector per trip the NVLS variant was latency-bound.
   constexpr int U = (MODE == MODE_NVLS) ? 4 : 2;
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x * U + threadIdx.x; i0 < lim; i0 += gstride() * U) {
     float gg[U][N];

@@ -1,4 +1,4 @@
-// b200mpi device-side primitives (sm_100a).
+// b200mpi device-side primitives (sm_90a).
 //
 // Everything a collective kernel needs that is not the loop itself: the
 // per-rank device context, .sys-scoped flag signalling between same-index CTAs
@@ -30,7 +30,7 @@ constexpr size_t kEpochWords = 2 * (size_t)kMaxBlocks;
 //   signal pad  : [kSigWords, kSigWords + 4*kPipeLanes*kMaxRanks)  IN-ready / REDUCED / DONE / ENTRY flags, [kind][lane][src rank]
 //   epoch array : [kEpochWords, kEpochWords + 4*kPipeLanes)        chunks done so far per (role, lane), then the
 //                                                                  local copy-out counter the copy-in CTA polls
-constexpr int kPipeLanes = 48;
+constexpr int kPipeLanes = 44;           // 3 x 44 = 132 CTAs: one per H100 SM, so every lane is co-resident
 constexpr size_t kPipeSigOff = kSigWords;
 constexpr size_t kPipeSigWords = 4 * (size_t)kPipeLanes * kMaxRanks;
 constexpr size_t kSigWordsTotal = kSigWords + kPipeSigWords;

@@ -1,27 +1,25 @@
-// 1x1-convolution GEMM with BatchNorm statistics fused into the epilogue (sm_100a: TMA + tcgen05 + TMEM).
+// 1x1-convolution GEMM with BatchNorm statistics fused into the epilogue (sm_90a: TMA + wgmma + mbarrier).
 //
-//   Y[M,N] = X[M,K] . W[N,K]^T      bf16 in, fp32 accumulate in TMEM, bf16 out   (NHWC activations: M = N*H*W, K = Cin,
-//                                                                                  N = Cout, W is the conv weight as stored)
+//   Y[M,N] = X[M,K] . W[N,K]^T      bf16 in, fp32 accumulate in registers, bf16 out   (NHWC activations: M = N*H*W,
+//                                                                                       K = Cin, N = Cout, W is the conv
+//                                                                                       weight as stored)
 //   partials[p][2n+0] += sum_m Y[m,n],  partials[p][2n+1] += sum_m Y[m,n]^2      (one row per CTA m-group, the layout the
 //                                                                                  BN finalize kernel of bn_act.cu merges)
 //
 // Why: two thirds of ResNet's BatchNorm layers follow a 1x1 convolution. Their statistics pass re-reads the whole
-// convolution output from HBM (profiles/launches_resnet101_step_fusedbn.md: k_bn_fwd_stats = 6.7 % of the step); here the
-// tile is still in shared memory when its column sums are taken, so the pass disappears. The reference has no kernels at
-// all (SURVEY.md §2.2) — this is part of the data plane the new framework adds.
+// convolution output from HBM; here the tile is still in shared memory when its column sums are taken, so the pass
+// disappears. The reference has no kernels at all (SURVEY.md §2.2) — this is part of the data plane the new framework adds.
 //
-// Structure (the canonical Blackwell GEMM: one warp per role, three pipelines):
-//   warp 0      TMA producer   : cp.async.bulk.tensor loads of the X and W tiles (128B swizzle) into a 4-stage ring
-//   warp 1      MMA issuer     : one lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16) into one of two TMEM
-//                                accumulators; tcgen05.commit releases smem stages / publishes the accumulator
-//   warps 2..5  epilogue       : tcgen05.ld (32 lanes x 32 columns per warp) -> bf16 -> swizzled smem staging ->
-//                                column sums from smem + TMA store of the tile; overlaps the next tile's main loop
-// Persistent: CTA c owns column block c % num_n and walks m-blocks with stride grid/num_n, so every epilogue thread keeps one
-// column's running sums in registers for the whole kernel and writes a single partial row at the end (no atomics).
-//
-// Status: first executed on a B200 in round 2 - numerics 10 / 10 against fp32 references (tests/test_zz_gemm_bnstats_gpu.py),
-// ncu capture + 12-shape micro-benchmark in profiles/ncu_gemm_bnstats.md, ResNet-101 step 14.15 -> 13.75 ms; on by default
-// for eligible 1x1 convolutions (B200MPI_FUSED_CONV1X1=0 restores cuDNN). Every wait is bounded and traps instead of hanging.
+// Structure (warp-specialised Hopper GEMM):
+//   warp 8        TMA producer : cp.async.bulk.tensor loads of the X and W tiles (128B swizzle) into a 4-stage ring
+//   warps 0..7    two consumer warpgroups; warpgroup g owns rows [64g, 64g+64) of the 128-row tile:
+//                   wgmma.mma_async m64nBNk16 (bf16 x bf16 -> fp32 registers), one k-block in flight, each finished
+//                   k-block releases its stage to the producer; then registers -> bf16 -> swizzled smem staging ->
+//                   TMA store of the tile + column sums of the warpgroup's 64 rows from smem
+// The producer runs ahead into the next tile while the consumers are in the epilogue.
+// Persistent: CTA c owns column block c % num_n and walks m-blocks with stride grid/num_n, so every consumer thread keeps
+// one column's running sums in registers for the whole kernel; the two warpgroups' sums are added in shared memory and
+// a single partial row is written at the end (no atomics). Every wait is bounded and traps instead of hanging.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -33,9 +31,10 @@
 namespace b200mpi {
 namespace gemm {
 
-constexpr int kThreads = 192;    // 6 warps: TMA, MMA, 4 x epilogue
-constexpr int kEpiThreads = 128;
-constexpr uint32_t kABytes = BM * BK * 2;   // 16 KiB
+constexpr int kConsumers = 256;              // two warpgroups
+constexpr int kThreads = kConsumers + 32;    // + the TMA producer warp
+constexpr int kMaxParts = 132;               // partial rows: at most one per SM (H100 SXM: 132 SMs)
+constexpr uint32_t kABytes = BM * BK * 2;    // 16 KiB
 constexpr long long kTimeoutCycles = 6000000000LL;  // ~3 s: a broken pipeline traps instead of hanging the GPU
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -86,53 +85,66 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// ----------------------------------------------------------------- tcgen05 ----
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (cute/arch/mma_sm100_desc.hpp: SmemDescriptor):
+// ------------------------------------------------------------------- wgmma ----
+// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle (cute/arch/mma_sm90_desc.hpp: GmmaDescriptor):
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (=1: unused for swizzled K-major) |
-//   [32,46) stride byte offset >> 4 (=64: 8 rows x 128 B between core-matrix groups) | [46,48) version = 1 (sm_100) |
-//   [61,64) layout = 2 (SWIZZLE_128B)
+//   [32,46) stride byte offset >> 4 (=64: 8 rows x 128 B between core-matrix groups) | [49,52) base offset = 0 (every
+//   operand tile starts on a 1024-byte swizzle atom) | [62,64) layout = 1 (SWIZZLE_128B)
 __host__ __device__ __forceinline__ uint64_t make_desc_kmajor_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)64 << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)64 << 32) | ((uint64_t)1 << 62);
 }
-// Instruction descriptor (InstrDescriptor): c_format F32 (1) at [4,6), a/b format BF16 (1) at [7,10)/[10,13),
-// a/b K-major (0) at 15/16, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x BN] (+)= A[64 x 16] . B[BN x 16]^T, both operands K-major in swizzled smem. Accumulator fragment of thread
+// (warp w of the warpgroup, lane l): d[4j + 2i + c] = D[16w + l/4 + 8i][8j + 2(l%4) + c]
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
+      "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t"
       "}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
+
+template <>
+__device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
+      "%25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cons_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
 
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory"); }
-
-__device__ __forceinline__ uint32_t pack_bf16(uint32_t lo_f32_bits, uint32_t hi_f32_bits) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(__uint_as_float(lo_f32_bits), __uint_as_float(hi_f32_bits));
+__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
@@ -145,9 +157,9 @@ struct Smem {
   static constexpr uint32_t kA = 0;
   static constexpr uint32_t kB = kStages * kABytes;
   static constexpr uint32_t kOut = kB + kStages * kBBytes;
-  static constexpr uint32_t kBars = kOut + kOutBytes;             // full[S], empty[S], tmem_full[2], tmem_empty[2]
-  static constexpr uint32_t kTmemSlot = kBars + (2 * kStages + 4) * 8;
-  static constexpr uint32_t kTotal = kTmemSlot + 16;
+  static constexpr uint32_t kSums = kOut + kOutBytes;             // [BN][2] fp32: warpgroup 1's column sums
+  static constexpr uint32_t kBars = kSums + BN * 8;               // full[S], empty[S]
+  static constexpr uint32_t kTotal = kBars + 2 * kStages * 8;
   static constexpr uint32_t kDynamic = kTotal + 1024;             // slack to align the base to 1024 B (swizzle atoms)
 };
 
@@ -156,16 +168,13 @@ __global__ void __launch_bounds__(kThreads, 1)
 k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmY,
                float* __restrict__ partials, int M, int N, int K, int num_n) {
   using L = Smem<BN>;
-  constexpr uint32_t kTmemCols = 2 * BN;  // two accumulators; 128 or 256: a power of two >= 32
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t sA = base + L::kA, sB = base + L::kB, sOut = base + L::kOut, sBar = base + L::kBars;
+  float* sums = reinterpret_cast<float*>(base_ptr + L::kSums);
   auto full_bar = [&](int s) { return sBar + 8u * s; };
   auto empty_bar = [&](int s) { return sBar + 8u * (kStages + s); };
-  auto tfull_bar = [&](int a) { return sBar + 8u * (2 * kStages + a); };
-  auto tempty_bar = [&](int a) { return sBar + 8u * (2 * kStages + 2 + a); };
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(base_ptr + L::kTmemSlot);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const TileWalk walk((int)blockIdx.x, (int)gridDim.x, num_n, M);
@@ -173,33 +182,20 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const int num_k = K / BK;
   const int n0 = walk.n_blk * BN;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumers / 32 && lane == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmY);
-  }
-  if (warp == 1) {  // TMEM allocation: one full warp; the same warp frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(base + L::kTmemSlot), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (warp == 2 && lane == 0) {
     for (int s = 0; s < kStages; s++) {
-      mbar_init(full_bar(s), 1);    // producer's arrive.expect_tx (+ the TMA transaction bytes)
-      mbar_init(empty_bar(s), 1);   // tcgen05.commit of the MMAs that read the stage
-    }
-    for (int a = 0; a < 2; a++) {
-      mbar_init(tfull_bar(a), 1);   // tcgen05.commit after the tile's last MMA
-      mbar_init(tempty_bar(a), 4);  // one arrive per epilogue warp
+      mbar_init(full_bar(s), 1);                   // producer's arrive.expect_tx (+ the TMA transaction bytes)
+      mbar_init(empty_bar(s), kConsumers / 32);    // one arrive per consumer warp once its wgmma has read the stage
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kConsumers / 32) {
     // ===================================================== TMA producer ====
     if (lane == 0) {
       Ring st;
@@ -213,97 +209,84 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         }
       }
     }
-    __syncwarp();   // lanes 1..31 skipped the loop: reconverge before the block-wide barrier below
-  } else if (warp == 1) {
-    // ======================================================= MMA issuer ====
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BM, BN);
-      Ring st, acc;
-      for (int m_blk = m_first; m_blk < num_m; m_blk += m_step) {
-        mbar_wait(tempty_bar(acc.s), acc.ph ^ 1u);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(acc.s * BN);
-        for (int kb = 0; kb < num_k; kb++) {
-          mbar_wait(full_bar(st.s), st.ph);
-          tc_fence_after();
-          const uint64_t adesc = make_desc_kmajor_sw128(sA + st.s * kABytes);
-          const uint64_t bdesc = make_desc_kmajor_sw128(sB + st.s * L::kBBytes);
+    return;
+  }
+
+  // =========================================================== consumers ====
+  const int ct = threadIdx.x;                  // 0..255
+  const int wg = warp >> 2;                    // rows [64 wg, 64 wg + 64) of every tile
+  const int t = ct & 127;                      // thread `t` of each warpgroup owns column n0 + t for the statistics
+  const bool col_owner = t < BN;
+  const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  float s1 = 0.f, s2 = 0.f;
+  float d[BN / 2] = {};
+  Ring st;
+  for (int m_blk = m_first; m_blk < num_m; m_blk += m_step) {
+    int prev = 0;
+    for (int kb = 0; kb < num_k; kb++) {
+      mbar_wait(full_bar(st.s), st.ph);
+      wgmma_fence();
+      const uint64_t adesc = make_desc_kmajor_sw128(sA + st.s * kABytes + (uint32_t)wg * 64u * 128u);
+      const uint64_t bdesc = make_desc_kmajor_sw128(sB + st.s * L::kBBytes);
 #pragma unroll
-          for (int k = 0; k < BK / UMMA_K; k++)  // +32 bytes along K inside the swizzle atom = +2 in the address field
-            umma_bf16(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-          umma_commit(empty_bar(st.s));        // stage reusable once these MMAs have read it
-          st.advance(kStages);
-        }
-        umma_commit(tfull_bar(acc.s));         // accumulator complete
-        acc.advance(2);
+      for (int k = 0; k < BK / MMA_K; k++)  // +32 bytes along K inside the swizzle atom = +2 in the address field
+        wgmma_bf16<BN>(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                         // the previous k-block's MMAs are done reading their stage
+      if (kb > 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar(prev));
       }
+      prev = st.s;
+      st.advance(kStages);
     }
+    wgmma_wait<0>();
     __syncwarp();
-  } else {
-    // ========================================================= epilogue ====
-    const int et = threadIdx.x - 64;             // 0..127
-    const int q = warp & 3;                      // TMEM lane quarter this warp may access: lanes [32q, 32q+32)
-    const int row = q * 32 + lane;               // tile row held by this thread
-    const bool col_owner = et < BN;              // thread `et` owns column n0 + et for the statistics
-    float s1 = 0.f, s2 = 0.f;
-    Ring acc;
-    for (int m_blk = m_first; m_blk < num_m; m_blk += m_step) {
-      if (et == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous tile's store has read the staging
-      epi_bar_sync();
-      mbar_wait(tfull_bar(acc.s), acc.ph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc.s * BN);
+    if (lane == 0) mbar_arrive(empty_bar(prev));
+
+    if (ct == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous tile's store has read the staging
+    cons_bar_sync();                                                               // ... and its column sums are taken
+    // fp32 fragment -> bf16 pairs in the swizzled staging layout (gemm_bnstats_logic.h)
 #pragma unroll
-      for (int c = 0; c < BN / 32; c++) {
-        uint32_t v[32];
-        tmem_ld_32x32(taddr + (uint32_t)(c * 32), v);
-        tmem_ld_wait();
-        // 32 fp32 -> 32 bf16 = 4 groups of 16 B in the swizzled staging layout (gemm_bnstats_logic.h)
+    for (int j = 0; j < BN / 8; j++) {
+      const int col = 8 * j + 2 * (lane & 3);
 #pragma unroll
-        for (int g = 0; g < 4; g++) {
-          const uint32_t dst = sOut + stage_group_byte(row, c, g);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pack_bf16(v[8 * g + 0], v[8 * g + 1])),
-                       "r"(pack_bf16(v[8 * g + 2], v[8 * g + 3])), "r"(pack_bf16(v[8 * g + 4], v[8 * g + 5])),
-                       "r"(pack_bf16(v[8 * g + 6], v[8 * g + 7]))
-                       : "memory");
-        }
+      for (int i = 0; i < 2; i++) {
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sOut + stage_elem_byte(col, frag_row + 8 * i)),
+                     "r"(pack_bf16(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]))
+                     : "memory");
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc.s));  // accumulator free for the MMA warp (tile after next)
-      acc.advance(2);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA store
-      epi_bar_sync();
-      if (et == 0) {
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA store
+    cons_bar_sync();
+    if (ct == 0) {
 #pragma unroll
-        for (int b = 0; b < (int)L::kOutBoxes; b++) tma_store_2d(&tmY, sOut + (uint32_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      }
-      if (col_owner) {
-        // column sums of the bf16-rounded tile (what the BN apply pass will read back). Rows past M are zero-filled by TMA.
+      for (int b = 0; b < (int)L::kOutBoxes; b++) tma_store_2d(&tmY, sOut + (uint32_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
+      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+    if (col_owner) {
+      // column sums of the bf16-rounded tile (what the BN apply pass will read back). Rows past M are zero-filled by TMA.
 #pragma unroll 8
-        for (int r = 0; r < BM; r++) {
-          uint16_t h;
-          asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(sOut + stage_elem_byte(et, r)));
-          const float f = __uint_as_float((uint32_t)h << 16);
-          s1 += f;
-          s2 = fmaf(f, f, s2);
-        }
+      for (int r = wg * 64; r < wg * 64 + 64; r++) {
+        uint16_t h;
+        asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(sOut + stage_elem_byte(t, r)));
+        const float f = __uint_as_float((uint32_t)h << 16);
+        s1 += f;
+        s2 = fmaf(f, f, s2);
       }
     }
-    if (col_owner && m_first < num_m) {
-      float* row_out = partials + partial_index(m_first, N, n0 + et);
-      row_out[0] = s1;
-      row_out[1] = s2;
-    }
-    if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores landed before the CTA exits
-    tc_fence_before();
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
+  if (wg == 1 && col_owner) {
+    sums[2 * t] = s1;
+    sums[2 * t + 1] = s2;
   }
+  cons_bar_sync();
+  if (wg == 0 && col_owner && m_first < num_m) {
+    float* row_out = partials + partial_index(m_first, N, n0 + t);
+    row_out[0] = s1 + sums[2 * t];
+    row_out[1] = s2 + sums[2 * t + 1];
+  }
+  if (ct == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores landed before the CTA exits
 }
 
 // ------------------------------------------------------------------- host ----
@@ -339,7 +322,7 @@ static int sm_count() {
   if (!n) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kMaxParts;
   }
   return n;
 }
@@ -351,7 +334,7 @@ static int launch(const void* X, const void* W, void* Y, float* partials, int* p
       !make_map(&tmY, Y, (uint64_t)M, (uint64_t)N, BM))
     return B200MPI_ERR_CUDA;
   const int num_n = N / BN, num_m = (int)((M + BM - 1) / BM);
-  int groups = sm_count() / num_n;
+  int groups = (sm_count() < kMaxParts ? sm_count() : kMaxParts) / num_n;
   if (groups < 1) return B200MPI_ERR_UNSUPPORTED;
   if (groups > num_m) groups = num_m;
   static bool attr_set = false;
@@ -374,11 +357,11 @@ extern "C" {
 // problems (a 2x2 feature map at batch 4) are latency-bound anyway and stay with the library.
 int b200mpi_gemm_bnstats_supported(long long M, int N, int K) {
   return (M >= 128 && M < (1LL << 31) - 128 && N >= 64 && N % 64 == 0 && K >= 64 && K % 64 == 0 &&
-          N / (N % 128 == 0 ? 128 : 64) <= 148) ? 1 : 0;
+          N / (N % 128 == 0 ? 128 : 64) <= b200mpi::gemm::kMaxParts) ? 1 : 0;
 }
 
 // rows of per-column {sum, sum of squares} the kernel may write: one per m-group, at most one per SM
-size_t b200mpi_gemm_bnstats_partial_floats(int N) { return (size_t)148 * 2 * (size_t)N; }
+size_t b200mpi_gemm_bnstats_partial_floats(int N) { return (size_t)b200mpi::gemm::kMaxParts * 2 * (size_t)N; }
 
 // Y = X . W^T (bf16, row-major, X [M,K], W [N,K], Y [M,N], all 16-byte aligned) and partials[parts][2N]; *parts = rows written.
 int b200mpi_gemm_bnstats(const void* X, const void* W, void* Y, float* partials, int* parts, long long M, int N, int K, void* stream) {

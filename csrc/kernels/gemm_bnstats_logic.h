@@ -1,4 +1,4 @@
-// Index and phase arithmetic of the tcgen05 GEMM + BN-statistics kernel (gemm_bnstats.cu), shared verbatim between the
+// Index and phase arithmetic of the wgmma GEMM + BN-statistics kernel (gemm_bnstats.cu), shared verbatim between the
 // kernel and its host model (csrc/tests/gemm_pipeline_model.cc): pipeline ring state, persistent tile walk, the
 // 128-byte-swizzled layout of the output staging buffer and the addressing of the per-CTA partial rows.
 #pragma once
@@ -14,9 +14,9 @@
 namespace b200mpi {
 namespace gemm {
 
-constexpr int BM = 128;          // rows per tile == TMEM lanes == UMMA M
+constexpr int BM = 128;          // rows per tile: two warpgroups x wgmma M = 64
 constexpr int BK = 64;           // 64 bf16 = 128 bytes = one swizzle-128B row
-constexpr int UMMA_K = 16;       // K per tcgen05.mma for 16-bit inputs
+constexpr int MMA_K = 16;        // K per wgmma.mma_async for 16-bit inputs
 constexpr int kStages = 4;
 constexpr uint32_t kBoxBytes = BM * 128;   // one TMA store box: 128 rows x 64 bf16
 

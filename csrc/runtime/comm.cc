@@ -1,7 +1,7 @@
 // b200mpi communicator: peer-memory windows (CUDA VMM + NVLS multicast, cudaIpc
 // fallback), algorithm selection, kernel launch plumbing and the C ABI.
 //
-// Reference parity: SURVEY.md §5.9 (B200-native replacement for the
+// Reference parity: SURVEY.md §5.9 (GPU-native replacement for the
 // Horovod -> NCCL data plane the reference launches but does not contain).
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -148,7 +148,7 @@ struct b200mpi_comm {
   size_t oneshot_max = 256 << 10;
   size_t nvls_min = 0;
   int max_blocks = 64;
-  int nvls_blocks = 16;  // the switch does the adds: 16 CTAs saturate NVLS (sweep: nvls@16 >= nvls@32 > nvls@128)
+  int nvls_blocks = 16;  // the switch does the adds, so few CTAs are needed (not yet swept on H100)
   int timeout_ms = 30000;
   // pipelined staged allreduce (user pointers): from pipe_min bytes up; lanes per mode (each lane = 3 CTAs)
   size_t pipe_min = (size_t)8 << 20;
@@ -156,13 +156,12 @@ struct b200mpi_comm {
   int pipe_p2p = 0;
   size_t pipe_chunk = (size_t)1 << 20;
   // user-pointer allreduce with NVLS available: below this size the registered zero-copy two-shot is preferred to the staging
-  // pipeline. As a kernel it is faster up to 128 MiB (8 GPUs: 60.8 vs 83.6 us at 16 MiB, 386 vs 386 at 128 MiB, 747 vs 696 at
-  // 256 MiB), but every call on the registered path pays a host agreement round (two rendezvous allgathers, reg_exchange) that
-  // graph-replay timings do not show and that the eager callers of this path (torch DDP buckets under the shim) would pay per
-  // bucket. The end-to-end DDP measurement of round 2 (28.9 k img/s, 8 GPUs) ran on the pipeline: 0 = keep that.
+  // pipeline. As a kernel it can be faster at mid sizes, but every call on the registered path pays a host agreement round (two
+  // rendezvous allgathers, reg_exchange) that graph-replay timings do not show and that the eager callers of this path (torch
+  // DDP buckets under the shim) would pay per bucket: 0 = always the pipeline. Not yet measured on H100.
   size_t pipe_pref_min = 0;
-  // reduce-scatter: the registered pull (630 GB/s-class kernel at 4 and 8 GPUs) instead of the NVLS pipeline (564 GB/s at 8 GPUs,
-  // NCCL 632) once the message is large enough for the host agreement round (~50 us) to disappear next to the kernel time
+  // reduce-scatter: the registered pull instead of the NVLS pipeline once the message is large enough for the host agreement
+  // round to disappear next to the kernel time (threshold not yet measured on H100)
   size_t rs_reg_min = (size_t)64 << 20;
   // lazy registration of user buffers (cudaIpc): peer mappings by (rank, allocation id); see reg_exchange()
   size_t reg_min = (size_t)8 << 20;
@@ -451,7 +450,7 @@ static void window_release(b200mpi_comm* c, Window& W) {
 // --------------------------------------------------------------- set-up ----
 static int comm_finish_init(b200mpi_comm* c, size_t staging_bytes) {
   c->timeout_ms = env_int("B200MPI_TIMEOUT_MS", 30000);
-  // Crossovers measured on 8xB200 / NVSwitch (profiles/allreduce_sweep_n{2,8}_f32.json):
+  // Crossovers by world size (not yet measured on H100; benchmarks/allreduce_sweep.py + autotune.py re-derive them):
   //  world 2 : push one-shot wins to 1 MiB, then P2P two-shot; NVLS never pays (1.5 S vs 1.0 S link bytes)
   //  world 8 : one-shot to 64 KiB, NVLS above (S(1+1/N) vs 2S(N-1)/N link bytes per direction)
   if (c->world <= 2) { c->oneshot_max = (size_t)1 << 20; c->nvls_min = (size_t)-1; }
@@ -477,7 +476,7 @@ static int comm_finish_init(b200mpi_comm* c, size_t staging_bytes) {
   c->pipe_pref_min = env_size("B200MPI_PIPE_PREF_MIN_BYTES", c->pipe_pref_min);
   c->rs_reg_min = env_size("B200MPI_RS_REG_MIN_BYTES", c->rs_reg_min);
   c->reg_mode = env_int("B200MPI_REG", c->reg_mode);
-  // 16 MiB one-shot region + 144 MiB for the pipelined kernels (48 lanes x 3 slots x 1 MiB)
+  // 16 MiB one-shot region + 144 MiB for the pipelined kernels (44 lanes x 3 slots x 1 MiB = 132 MiB, plus slack)
   if (staging_bytes == 0) staging_bytes = env_size("B200MPI_STAGING_BYTES", c->local ? (size_t)64 << 20 : (size_t)160 << 20);
   // one-shot region: 2 parities x kOneshotBlocks CTAs x kMaxRanks slots x cap
   c->oneshot_cap_vecs = 2048;  // 32 KiB per slot -> 1 MiB max one-shot payload
@@ -1284,9 +1283,8 @@ int b200mpi_reduce_scatter(b200mpi_comm_t c, const void* in, void* out, size_t c
   if (dtype < 0 || dtype > 2 || op < 0 || op > 2) return fail(B200MPI_ERR_INVALID, "reduce_scatter: bad dtype/op");
   const bool rs_nvls = c->multicast && (op == B200MPI_SUM || dtype != B200MPI_F32);
   // zero-copy: pull the owned block from every input. Without NVLS always; with NVLS from rs_reg_min bytes of input up: the P2P
-  // pull runs at the link's read rate (allreduce_reg: 630 GB/s at 4 and 8 GPUs) with no staging copy of the N x larger input,
-  // the pipelined kernel reached 564 GB/s at 8 GPUs against NCCL's 632 (profiles/r2/roofline_shim_vs_nccl_n8.md); below that
-  // size the per-call host agreement of the registered path would cost more than the kernel gains
+  // pull runs at the link's read rate with no staging copy of the N x larger input; below that size the per-call host
+  // agreement of the registered path would cost more than the kernel gains
   if (total % 16 == 0 && reg_wanted(c, total * c->world, !rs_nvls || total * c->world >= c->rs_reg_min)) {
     Win win_in, win_out;
     if (reg_exchange(c, in, out, total * c->world, total, true, &win_in, &win_out) == REG_IPC) {

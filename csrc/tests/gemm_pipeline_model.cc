@@ -1,9 +1,9 @@
-// Host model of the tcgen05 GEMM + BN-statistics kernel (csrc/kernels/gemm_bnstats.cu).
+// Host model of the wgmma GEMM + BN-statistics kernel (csrc/kernels/gemm_bnstats.cu).
 //
-// The kernel's three warp roles run here as threads of one "CTA", with the hardware pieces replaced by small host
-// emulations — mbarriers (arrival count + transaction bytes + phase parity), TMA loads and stores (tile copies in the
-// 128-byte-swizzled shared-memory layout, zero fill / clipping at the matrix edge), tcgen05.mma (fp32 accumulation of
-// K=16 slices into a two-buffer "TMEM"), tcgen05.commit (arrive when the issued MMAs are done: immediately), tcgen05.ld.
+// The kernel's roles (one TMA producer, two consumer warpgroups) run here as threads of one "CTA", with the hardware
+// pieces replaced by small host emulations — mbarriers (arrival count + transaction bytes + phase parity), TMA loads and
+// stores (tile copies in the 128-byte-swizzled shared-memory layout, zero fill / clipping at the matrix edge), and
+// wgmma.mma_async (fp32 accumulation of K=16 slices into the warpgroup's 64-row register fragment; complete on issue).
 // Everything that is arithmetic rather than hardware — ring/phase bookkeeping, the persistent tile walk, the swizzled
 // staging layout, column ownership, the partial-row addressing — is the SAME code as in the kernel
 // (csrc/kernels/gemm_bnstats_logic.h); the role loops are transcribed statement by statement from the kernel.
@@ -11,7 +11,7 @@
 // sum / sum of squares merged over the partial rows. A protocol error shows up as a deadlock (watchdog) or wrong data.
 //
 // What this cannot tell: whether the PTX wrappers mean what the model assumes (descriptor bits are cross-checked with
-// CuTe in umma_desc_test.cu). `make test_gemm_model`; run by tests/test_native_cpu.py.
+// CuTe in gmma_desc_test.cu). `make test_gemm_model`; run by tests/test_native_cpu.py.
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -84,21 +84,22 @@ struct Problem {
 };
 
 // ------------------------------------------------------------------- CTA ----
+constexpr int kConsumerWarps = 8;                    // empty-barrier arrivals per stage: one per consumer warp
+
 struct CTA {
   Problem& p;
   const int cta, grid, num_n;
   const int BN;
   std::vector<uint8_t> sA, sB, sOut;                 // kStages x tile, kStages x tile, BN/64 boxes
-  MBar full[kStages], empty[kStages], tfull[2], tempty[2];
-  std::vector<float> tmem;                           // [2][BM][BN]
-  NamedBarrier epi{4};                               // four epilogue warps (each modelled by one thread)
+  std::vector<float> sums;                           // [BN][2]: warpgroup 1's column sums
+  MBar full[kStages], empty[kStages];
+  NamedBarrier cons{2};                              // bar.sync 1, 256: the two consumer warpgroups (one thread each)
   std::mutex store_mu;                               // the TMA store "bulk group": finished when it returns
 
   CTA(Problem& p_, int cta_, int grid_, int num_n_)
       : p(p_), cta(cta_), grid(grid_), num_n(num_n_), BN(p_.BN), sA((size_t)kStages * BM * 128), sB((size_t)kStages * p_.BN * 128),
-        sOut((size_t)(p_.BN / 64) * kBoxBytes), tmem((size_t)2 * BM * p_.BN) {
-    for (int s = 0; s < kStages; s++) { full[s].reset(1); empty[s].reset(1); }
-    for (int a = 0; a < 2; a++) { tfull[a].reset(1); tempty[a].reset(4); }
+        sOut((size_t)(p_.BN / 64) * kBoxBytes), sums((size_t)2 * p_.BN, 0.f) {
+    for (int s = 0; s < kStages; s++) { full[s].reset(1); empty[s].reset(kConsumerWarps); }
   }
 
   // cp.async.bulk.tensor.2d load with SWIZZLE_128B: box of `rows` x 64 elements at (row0, k0), zero fill outside the matrix
@@ -121,23 +122,23 @@ struct CTA {
         p.Y[(size_t)(row0 + r) * p.N + col0 + j] = v;
       }
   }
-  // tcgen05.mma kind::f16, M=128, N=BN, K=16: D (+)= A[128 x 16] . B[BN x 16]^T, operands K-major in swizzled smem,
-  // `kbyte` = the +32 B per UMMA_K the kernel adds to the descriptor start address
-  void umma(float* d, const uint8_t* a, const uint8_t* b, int kslice, bool accumulate) {
-    for (int m = 0; m < BM; m++)
+  // wgmma m64nBNk16: D[64 x BN] (+)= A[64 x 16] . B[BN x 16]^T, A = rows [64 wg, 64 wg + 64) of the swizzled stage
+  void wgmma(float* d, const uint8_t* a, const uint8_t* b, int wg, int kslice, bool accumulate) {
+    for (int m = 0; m < 64; m++)
       for (int n = 0; n < BN; n++) {
         float acc = accumulate ? d[(size_t)m * BN + n] : 0.f;
-        for (int k = 0; k < UMMA_K; k++) {
+        for (int k = 0; k < MMA_K; k++) {
           uint16_t av, bv;
-          memcpy(&av, a + operand_elem_byte(m, kslice * UMMA_K + k), 2);
-          memcpy(&bv, b + operand_elem_byte(n, kslice * UMMA_K + k), 2);
+          memcpy(&av, a + operand_elem_byte(wg * 64 + m, kslice * MMA_K + k), 2);
+          memcpy(&bv, b + operand_elem_byte(n, kslice * MMA_K + k), 2);
           acc += bf2f(av) * bf2f(bv);
         }
         d[(size_t)m * BN + n] = acc;
       }
   }
+  void release(int s) { for (int w = 0; w < kConsumerWarps / 2; w++) empty[s].arrive(); }   // lane 0 of each warp
 
-  void producer() {  // warp 0, lane 0
+  void producer() {  // warp 8, lane 0
     const TileWalk walk(cta, grid, num_n, p.M);
     const int num_k = p.K / BK, n0 = walk.n_blk * BN;
     Ring st;
@@ -150,75 +151,65 @@ struct CTA {
         st.advance(kStages);
       }
   }
-  void mma() {  // warp 1, lane 0
+  // one consumer warpgroup; its 128 threads are executed one after the other between barriers
+  void consumer(int wg) {
     const TileWalk walk(cta, grid, num_n, p.M);
-    const int num_k = p.K / BK;
-    Ring st, acc;
+    const int num_k = p.K / BK, n0 = walk.n_blk * BN;
+    std::vector<float> d((size_t)64 * BN);               // the warpgroup's accumulator fragments
+    std::vector<float> s1(BN, 0.f), s2(BN, 0.f);         // registers of the column owners t < BN
+    Ring st;
     for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step) {
-      tempty[acc.s].wait(acc.ph ^ 1u);
-      float* d = tmem.data() + (size_t)acc.s * BM * BN;
+      int prev = 0;
       for (int kb = 0; kb < num_k; kb++) {
         full[st.s].wait(st.ph);
-        for (int k = 0; k < BK / UMMA_K; k++)
-          umma(d, sA.data() + (size_t)st.s * BM * 128, sB.data() + (size_t)st.s * BN * 128, k, (kb | k) != 0);
-        empty[st.s].arrive();   // tcgen05.commit -> empty
+        for (int k = 0; k < BK / MMA_K; k++)
+          wgmma(d.data(), sA.data() + (size_t)st.s * BM * 128, sB.data() + (size_t)st.s * BN * 128, wg, k, (kb | k) != 0);
+        if (kb > 0) release(prev);                         // wgmma.wait_group 1: the previous k-block is done
+        prev = st.s;
         st.advance(kStages);
       }
-      tfull[acc.s].arrive();    // tcgen05.commit -> tmem_full
-      acc.advance(2);
-    }
-  }
-  // one epilogue warp (warp index 2..5); its 32 lanes are executed one after the other between barriers
-  void epilogue(int warp, std::vector<float>& s1, std::vector<float>& s2) {
-    const TileWalk walk(cta, grid, num_n, p.M);
-    const int q = warp & 3, n0 = walk.n_blk * BN;
-    Ring acc;
-    for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step) {
-      // (et == 0: cp.async.bulk.wait_group.read 0 — the modelled store is synchronous)
-      epi.sync();
-      tfull[acc.s].wait(acc.ph);
-      const float* d = tmem.data() + (size_t)acc.s * BM * BN;
-      for (int lane = 0; lane < 32; lane++) {
-        const int row = q * 32 + lane;                       // TMEM lane quarter of this warp
-        for (int c = 0; c < BN / 32; c++)                    // tcgen05.ld 32x32b.x32: 32 consecutive columns of `row`
-          for (int g = 0; g < 4; g++) {
-            uint16_t packed[8];
-            for (int e = 0; e < 8; e++) packed[e] = f2bf(d[(size_t)row * BN + c * 32 + g * 8 + e]);
-            memcpy(sOut.data() + stage_group_byte(row, c, g), packed, 16);
+      release(prev);                                       // wgmma.wait_group 0
+      // (ct == 0: cp.async.bulk.wait_group.read 0 — the modelled store is synchronous)
+      cons.sync();
+      for (int w = 0; w < 4; w++)
+        for (int lane = 0; lane < 32; lane++) {
+          const int frag_row = wg * 64 + w * 16 + (lane >> 2);
+          for (int j = 0; j < BN / 8; j++) {
+            const int col = 8 * j + 2 * (lane & 3);
+            for (int i = 0; i < 2; i++) {
+              const int row = frag_row + 8 * i;
+              const uint16_t pair[2] = {f2bf(d[(size_t)(row - wg * 64) * BN + col]), f2bf(d[(size_t)(row - wg * 64) * BN + col + 1])};
+              memcpy(sOut.data() + stage_elem_byte(col, row), pair, 4);
+            }
           }
-      }
-      tempty[acc.s].arrive();                                // lane 0 of the warp
-      acc.advance(2);
-      epi.sync();
-      if (warp == 2) {                                       // et == 0 lives in the first epilogue warp
+        }
+      cons.sync();
+      if (wg == 0) {                                       // ct == 0 lives in warpgroup 0
         std::lock_guard<std::mutex> l(store_mu);
         for (int b = 0; b < BN / 64; b++) tma_store(sOut.data() + (size_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
       }
-      for (int lane = 0; lane < 32; lane++) {
-        const int et = (warp - 2) * 32 + lane;
-        if (et >= BN) continue;                              // col_owner
-        for (int r = 0; r < BM; r++) {
+      for (int t = 0; t < BN; t++)                         // col_owner
+        for (int r = wg * 64; r < wg * 64 + 64; r++) {
           uint16_t h;
-          memcpy(&h, sOut.data() + stage_elem_byte(et, r), 2);
+          memcpy(&h, sOut.data() + stage_elem_byte(t, r), 2);
           const float f = bf2f(h);
-          s1[et] += f;
-          s2[et] = std::fma(f, f, s2[et]);
+          s1[t] += f;
+          s2[t] = std::fma(f, f, s2[t]);
         }
+    }
+    if (wg == 1)
+      for (int t = 0; t < BN; t++) { sums[2 * t] = s1[t]; sums[2 * t + 1] = s2[t]; }
+    cons.sync();
+    if (wg == 0 && walk.m_first < walk.num_m)
+      for (int t = 0; t < BN; t++) {
+        p.partials[partial_index(walk.m_first, p.N, n0 + t)] = s1[t] + sums[2 * t];
+        p.partials[partial_index(walk.m_first, p.N, n0 + t) + 1] = s2[t] + sums[2 * t + 1];
       }
-    }
-    for (int lane = 0; lane < 32; lane++) {
-      const int et = (warp - 2) * 32 + lane;
-      if (et >= BN) continue;
-      p.partials[partial_index(walk.m_first, p.N, n0 + et)] = s1[et];
-      p.partials[partial_index(walk.m_first, p.N, n0 + et) + 1] = s2[et];
-    }
   }
   void run() {
-    std::vector<float> s1(128, 0.f), s2(128, 0.f);           // per-thread registers of the 128 epilogue threads
     std::vector<std::thread> th;
     th.emplace_back([&] { producer(); });
-    th.emplace_back([&] { mma(); });
-    for (int w = 2; w < 6; w++) th.emplace_back([&, w] { epilogue(w, s1, s2); });
+    for (int wg = 0; wg < 2; wg++) th.emplace_back([&, wg] { consumer(wg); });
     for (auto& t : th) t.join();
   }
 };

@@ -146,7 +146,7 @@ _atexit_registered = False
 
 def _start_engine(info, dev) -> None:
     """Native background engine (hvd/engine.py). Host tensors: on unless B200MPI_HVD_ENGINE=0. Device tensors: only with
-    B200MPI_HVD_ENGINE=1 (the GPU executor ran on 4 and 8 B200s in round 2; the direct path stays the default); it gets a communicator of its own because
+    B200MPI_HVD_ENGINE=1 (multi-GPU only, not yet run on H100; the direct path stays the default); it gets a communicator of its own because
     collectives on one communicator must be issued in the same order on every rank."""
     global _atexit_registered
     want = os.environ.get("B200MPI_HVD_ENGINE", "")

@@ -7,8 +7,7 @@ ranks: orthogonal gradients add, parallel gradients average. Two device paths:
 * ``B200MPI_ADASUM_KERNEL=1``: ``Communicator.adasum`` - ONE kernel per tensor (csrc/kernels/adasum.cu), each rank owns
   one slice of every vector, the tree levels run inside the launch over NVSwitch peer memory (S bytes pulled + S bytes
   pushed per rank, log2(N)+2 flag barriers). Power-of-two worlds, f32 / bf16 / f16, tensors up to
-  ``Communicator.adasum_max_bytes``. Opt-in: the kernel was written after this round's GPU budget was spent and has
-  not run on a B200 yet (tests/test_zzz_adasum_gpu.py is its numerics test).
+  ``Communicator.adasum_max_bytes``. Opt-in (tests/test_zzz_adasum_gpu.py is its numerics test).
 * otherwise every rank gathers the N tensors (one b200mpi allgather kernel) and folds the tree locally in fp32 -
   identical bits on all ranks, O(N*S) scratch; fine for the example-scale models that use Adasum.
 """

@@ -2,7 +2,7 @@
 tf_cnn_benchmarks ResNet-101, examples/v2beta1/tensorflow-benchmarks/
 tensorflow-benchmarks.yaml:38-42; Horovod MNIST, examples/v2beta1/horovod/
 tensorflow_mnist.py:38-73).  Model compute stays in PyTorch/cuDNN; the
-hand-written sm_100a surface is the collective + optimizer path."""
+hand-written sm_90a surface is the collective + optimizer path."""
 from .resnet import resnet18, resnet50, resnet101, resnet152, ResNet  # noqa: F401
 from .mnist import MnistConvNet  # noqa: F401
 from .classic import trivial, lenet, alexnet, vgg11, vgg16, vgg19  # noqa: F401

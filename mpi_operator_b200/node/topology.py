@@ -3,7 +3,7 @@
 The reference asks the Kubernetes API server where capacity is; a single-box
 daemon asks the hardware (BASELINE.json north-star).  Discovery order: NVML
 (``pynvml`` from nvidia-ml-py: device list, UUIDs, NVLink P2P status), then
-``torch.cuda``, then ``B200MPI_FAKE_GPUS=N`` for tests.  On HGX B200 every
+``torch.cuda``, then ``B200MPI_FAKE_GPUS=N`` for tests.  On an HGX H100 board every
 pair is an NVSwitch peer, so any k-of-8 placement is bandwidth-equivalent; we
 still record per-pair P2P capability and refuse non-peer placements.
 """

@@ -158,8 +158,8 @@ def bn_act(bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual: torch.Tensor = N
 
 # --------------------------------------------------------------------------------------------------------------
 # 1x1 convolution + BatchNorm(+residual)+ReLU with the BN statistics taken in the GEMM epilogue
-# (csrc/kernels/gemm_bnstats.cu: TMA + tcgen05 + TMEM). On by default since round 2 (numerics: tests/test_zz_gemm_bnstats_gpu.py
-# on a B200; ResNet-101 step 14.15 -> 13.75 ms, profiles/r2); B200MPI_FUSED_CONV1X1=0 keeps cuDNN for the 1x1 convolutions.
+# (csrc/kernels/gemm_bnstats.cu: TMA + wgmma). On by default (numerics: tests/test_zz_gemm_bnstats_gpu.py);
+# B200MPI_FUSED_CONV1X1=0 keeps cuDNN for the 1x1 convolutions.
 # Forward = 3 launches (GEMM+stats, finalize, apply) instead of conv + 3; backward = the fused BN backward kernels + two
 # library GEMMs (dgrad, wgrad).
 _CONV1X1 = os.environ.get("B200MPI_FUSED_CONV1X1", "1") == "1"
@@ -240,7 +240,7 @@ class _Conv1x1BNAct(torch.autograd.Function):
 def conv_bn_act(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual: torch.Tensor = None,
                 relu: bool = True) -> torch.Tensor:
     """``relu(bn(conv(x)) [+ residual])``. With B200MPI_FUSED_CONV1X1=1 an eligible 1x1 stride-1 convolution runs on the
-    tcgen05 GEMM whose epilogue already produces the BatchNorm statistics; everything else is ``bn_act(bn, conv(x), ...)``."""
+    wgmma GEMM whose epilogue already produces the BatchNorm statistics; everything else is ``bn_act(bn, conv(x), ...)``."""
     if (_CONV1X1 and _conv1x1_eligible(conv, bn, x)
             and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape[0] == x.shape[0]
                                       and residual.shape[1] == conv.out_channels and residual.shape[2:] == x.shape[2:]))):

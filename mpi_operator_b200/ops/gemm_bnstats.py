@@ -1,4 +1,4 @@
-"""Python front-end of the tcgen05 1x1-convolution GEMM with fused BatchNorm statistics
+"""Python front-end of the wgmma 1x1-convolution GEMM with fused BatchNorm statistics
 (csrc/kernels/gemm_bnstats.cu -> lib/libb200mpi_gemm.so).
 
     y, s1, s2 = conv1x1_with_stats(x, weight)
@@ -7,8 +7,8 @@
 (``conv.weight.view(Cout, Cin)``) in bf16. Returns the bf16 output [M, Cout] and the per-channel sum / sum of squares
 of that output (fp32), i.e. what BatchNorm's statistics pass would compute by re-reading ``y`` from HBM.
 
-EXPERIMENTAL: the kernel has been compiled for sm_100a but not yet executed on hardware (see the header of the .cu
-file); nothing in the default model path calls this module. The reference ships no kernels (SURVEY.md §2.2)."""
+The kernel is compiled for sm_90a (H100); ops/fused_bn.py calls it for eligible 1x1 convolutions. The reference ships no
+kernels (SURVEY.md §2.2)."""
 from __future__ import annotations
 
 import ctypes as C

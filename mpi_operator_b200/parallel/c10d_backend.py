@@ -6,7 +6,7 @@
     model = torch.nn.parallel.DistributedDataParallel(model)
 
 No preloading and no NCCL in the process: the process group is a Python ``ProcessGroup`` whose collectives call the same
-runtime the shim calls - ``runtime.comm.Communicator`` (sm_100a NVSwitch kernels, enqueued on the CURRENT CUDA stream, so the
+runtime the shim calls - ``runtime.comm.Communicator`` (sm_90a NVSwitch kernels, enqueued on the CURRENT CUDA stream, so the
 returned ``Work`` is complete in stream order exactly like ProcessGroupNCCL's) for CUDA tensors, the ``libmpi`` shim
 (``hvd.host_backend.HostCommunicator``) for CPU tensors. Reference call site that creates the obligation: the workloads of
 examples/v2beta1/tensorflow-benchmarks/tensorflow-benchmarks.yaml:26-42 reach their collectives through a framework-level

@@ -6,7 +6,7 @@ gradients, ``BroadcastGlobalVariablesHook(0)``; examples/v2beta1/horovod/
 tensorflow_mnist.py:133,143).  Horovod's engine = negotiate -> pack ready
 tensors into a fusion buffer -> ncclAllReduce -> scale -> unpack -> optimizer.
 
-B200-first redesign:
+GPU-first redesign:
 
 * parameters and gradients live *inside symmetric windows* (peer-mapped, NVLS
   bound): autograd writes gradients straight into NVLink-visible memory, so
@@ -56,8 +56,7 @@ class FlatModelState:
     parameters (conv / linear weights) become bf16 leaves that view it, their fp32 masters stay in
     the parameter window and the fused SGD kernel refreshes the shadow in the same pass
     (``lowp_win``). Forward then needs no per-layer fp32->bf16 weight cast and backward no
-    bf16->fp32 gradient cast + accumulate: ~3 small kernels per layer disappear from the step
-    (profiles/launches_resnet101_step_fusedbn.md: 13 % of device time in ATen elementwise kernels)."""
+    bf16->fp32 gradient cast + accumulate: ~3 small kernels per layer disappear from the step."""
 
     def __init__(self, module: nn.Module, comm: Communicator, bucket_bytes: int = 32 << 20, bf16_params: bool = False):
         self.comm = comm
@@ -192,8 +191,7 @@ class DataParallelTrainer:
         self.device = torch.device("cuda", comm.device) if comm.device != "cpu" else torch.device("cpu")
         self._cuda = self.device.type == "cuda"
         if bf16_params is None:
-            # Default on for single-GPU CUDA runs: ran on B200 in rounds 1 (driver XPASS) and 2 (profiles/r2: 15.34 -> 15.00
-            # ms/step). With world > 1 the fused kernel pushes the bf16 shadow to every peer with unicast 8-byte stores
+            # Default on for single-GPU CUDA runs (it removes the per-layer weight casts). With world > 1 the fused kernel pushes the bf16 shadow to every peer with unicast 8-byte stores
             # (no multimem form yet) and that path has not been measured on more than one GPU: opt-in there
             # (B200MPI_BF16_PARAMS=1). The CPU debug path keeps fp32 leaves unless asked.
             bf16_params = os.environ.get("B200MPI_BF16_PARAMS", "1" if (self._cuda and comm.world == 1) else "0") == "1"
@@ -225,14 +223,13 @@ class DataParallelTrainer:
         self._sync = True
         self._carry = False
         # B200MPI_ASYNC_H2D=1: inputs go host -> staging buffer on a copy stream (overlapping the previous step's compute),
-        # then device -> device into the graph's static input. Default on (profiles/r2: 15.34 -> 15.10 ms/step on 1 GPU;
-        # at 8 GPUs the compute-stream copy was the suspected scaling limiter, VERDICT round 1)
+        # then device -> device into the graph's static input, so the copy overlaps compute. Default on.
         self.async_h2d = os.environ.get("B200MPI_ASYNC_H2D", "1") == "1" if async_h2d is None else bool(async_h2d)
         self._copy_stream = torch.cuda.Stream(device=self.device) if (self.async_h2d and self._cuda) else None
         self._stage_x = self._stage_y = None
         self._pending_batch = None
-        # the 104 `num_batches_tracked += 1` kernels of a ResNet-101 step become one multi-tensor add (ran on a B200 in round 2
-        # together with the other flags: profiles/r2/bench_all_flags.json); B200MPI_DEFER_NBT=0 restores one add per BN layer
+        # the 104 `num_batches_tracked += 1` kernels of a ResNet-101 step become one multi-tensor add;
+        # B200MPI_DEFER_NBT=0 restores one add per BN layer
         self._defer_nbt = os.environ.get("B200MPI_DEFER_NBT", "1" if self._cuda else "0") == "1"
         self._graph_ops: list = []   # collectives recorded in the CUDA graph: replays launch them without the host
         self._replays = 0

@@ -29,7 +29,7 @@ class B200MPIError(RuntimeError):
 
 
 def build(force: bool = False) -> Path:
-    """Compile libb200mpi.so for sm_100a with nvcc (no GPU needed)."""
+    """Compile libb200mpi.so for sm_90a with nvcc (no GPU needed)."""
     if LIB_PATH.exists() and not force:
         srcs = list((_ROOT / "csrc").rglob("*.cu")) + list((_ROOT / "csrc").rglob("*.cc")) + \
             list((_ROOT / "csrc").rglob("*.h")) + list((_ROOT / "csrc").rglob("*.cuh"))

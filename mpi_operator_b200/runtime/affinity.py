@@ -1,6 +1,6 @@
 """CPU affinity next to a rank's GPU, for ranks that were not started by the in-tree ``mpirun`` (torchrun, a notebook, srun).
 
-On an 8xB200 HGX board GPUs 0-3 and 4-7 hang off different sockets. A rank whose host thread runs on the far socket first-touches
+On an 8-GPU HGX board GPUs 0-3 and 4-7 hang off different sockets. A rank whose host thread runs on the far socket first-touches
 its pinned staging buffers in far memory, and every H2D copy of the input batch then crosses the socket interconnect. Open MPI's
 answer is ``--bind-to numa`` (the reference's command lines say ``-bind-to none``, examples/v2beta1/tensorflow-benchmarks/
 tensorflow-benchmarks.yaml:23-24, which stays the default here); ``csrc/spawner/mpirun.cc`` implements that flag with GPU locality,

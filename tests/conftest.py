@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a real CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a real CUDA device (run on the H100 box)")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 CUDA devices")
 
 

@@ -92,8 +92,14 @@ def test_trace_export_and_roofline_report(tmp_path):
     ev = json.load(open(out))["traceEvents"]
     assert sum(1 for e in ev if e["ph"] == "X") == 3 and {e["pid"] for e in ev} == {0, 1}
     assert trace.summarize(trace.load_jsonl(str(p)))["allreduce[oneshot]"] == {"calls": 2, "bytes": 2048}
-    md = roofline.report("/root/repo/profiles/allreduce_sweep_n8_f32.json")
-    assert "| float32 | 1073741824 | nvls" in md and "x |" in md
+    sweep = tmp_path / "allreduce_sweep_n8_f32.json"
+    row = {"dtype": "float32", "bytes": 1 << 30}
+    sweep.write_text(json.dumps({"world": 8, "multicast": True, "rows": [
+        dict(row, algo="twoshot", ms_median_max_over_ranks=4.0, algbw_gbs=268.4, busbw_gbs=469.8),
+        dict(row, algo="nvls", ms_median_max_over_ranks=3.0, algbw_gbs=357.9, busbw_gbs=626.3),
+        dict(row, algo="nccl", ms_median_max_over_ranks=3.3, algbw_gbs=325.4, busbw_gbs=569.4)]}))
+    md = roofline.report(str(sweep))
+    assert "| float32 | 1073741824 | nvls | 3000.0 |" in md and "| 1.39 | 3300.0 | 569.4 | 1.10x |" in md
 
 
 def _repo():

@@ -266,19 +266,19 @@ def test_host_runtime_is_clean_under_address_and_ub_sanitizers():
     assert "ERROR: AddressSanitizer" not in r.stderr and "runtime error:" not in r.stderr
 
 
-def test_tcgen05_gemm_library_builds_loads_and_validates_shapes():
-    """libb200mpi_gemm.so (csrc/kernels/gemm_bnstats.cu) is cross-compiled for sm_100a by `make`; its shape contract is
-    checked on the host: N and K multiples of 64, at most 148 column blocks, M below 2^31."""
+def test_wgmma_gemm_library_builds_loads_and_validates_shapes():
+    """libb200mpi_gemm.so (csrc/kernels/gemm_bnstats.cu) is cross-compiled for sm_90a by `make`; its shape contract is
+    checked on the host: N and K multiples of 64, at most 132 column blocks (one per H100 SM), M below 2^31."""
     from mpi_operator_b200.ops import gemm_bnstats as g
     if not g.LIB_PATH.exists():
         pytest.skip("native libraries not built (run make)")
     assert g.supported(200704, 256, 64) and g.supported(128, 64, 64) and g.supported(50176, 2048, 512)
     assert not g.supported(128, 96, 64) and not g.supported(128, 64, 32) and not g.supported(0, 64, 64) and not g.supported(127, 64, 64)
-    assert not g.supported(128, 148 * 128 + 128, 64)
-    assert g.lib().b200mpi_gemm_bnstats_partial_floats(256) == 148 * 2 * 256
+    assert g.supported(128, 132 * 128, 64) and not g.supported(128, 132 * 128 + 128, 64)
+    assert g.lib().b200mpi_gemm_bnstats_partial_floats(256) == 132 * 2 * 256
     sass = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-sass", str(g.LIB_PATH)], capture_output=True, text=True)
-    if sass.returncode == 0:  # the tensor-core / TMA / TMEM instructions are really there
-        for mnemonic in ("UTCHMMA", "UTMALDG", "UTMASTG", "LDTM", "UTCBAR"):
+    if sass.returncode == 0:  # the warpgroup tensor-core and TMA instructions are really there
+        for mnemonic in ("HGMMA.64x128x16.F32.BF16", "HGMMA.64x64x16.F32.BF16", "UTMALDG", "UTMASTG", "WARPGROUP.ARRIVE"):
             assert mnemonic in sass.stdout, mnemonic
 
 
@@ -291,16 +291,16 @@ def test_runtime_launch_planning_on_the_host():
     assert r.returncode == 0 and "comm_host_test: all checks passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
-def test_tcgen05_descriptors_match_cute():
-    """`make test_umma_desc`: the instruction descriptor and the K-major / 128-byte-swizzle shared-memory descriptor packed by
-    hand in csrc/kernels/gemm_bnstats.cu are bit-identical to what CuTe builds for the same tile (host-only check)."""
+def test_wgmma_descriptors_match_cute():
+    """`make test_gmma_desc`: the K-major / 128-byte-swizzle wgmma shared-memory descriptor packed by hand in
+    csrc/kernels/gemm_bnstats.cu is bit-identical to what CuTe builds for the same tile (host-only check)."""
     import importlib.util
     spec = importlib.util.find_spec("flashinfer")   # located, not imported
     inc = os.path.join(os.path.dirname(spec.origin), "data", "cutlass", "include") if spec and spec.origin else ""
-    if not os.path.exists(os.path.join(inc, "cute", "arch", "mma_sm100_desc.hpp")):
+    if not os.path.exists(os.path.join(inc, "cute", "arch", "mma_sm90_desc.hpp")):
         pytest.skip("CUTLASS/CuTe headers not available")
-    r = subprocess.run(["make", "test_umma_desc"], cwd=REPO, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "umma_desc_test: descriptors match CuTe" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
+    r = subprocess.run(["make", "test_gmma_desc"], cwd=REPO, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and "gmma_desc_test: descriptors match CuTe" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
     assert "MISMATCH" not in r.stdout
 
 
@@ -314,11 +314,11 @@ def test_point_to_point_protocol_with_host_threads():
     assert r.returncode == 0 and "p2p_protocol_test: all checks passed" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
-def test_tcgen05_gemm_pipeline_host_model():
-    """`make test_gemm_model`: the three warp roles of csrc/kernels/gemm_bnstats.cu (TMA producer, MMA issuer, 4 epilogue warps)
-    as host threads over emulated mbarriers / TMA / TMEM, sharing the kernel's index and phase arithmetic
-    (gemm_bnstats_logic.h). Ring wrap-around, accumulator double buffering, ragged M, both tile widths, the swizzled staging
-    layout, column sums and partial rows are checked against a plain GEMM."""
+def test_wgmma_gemm_pipeline_host_model():
+    """`make test_gemm_model`: the roles of csrc/kernels/gemm_bnstats.cu (TMA producer warp, two consumer warpgroups) as
+    host threads over emulated mbarriers / TMA / wgmma, sharing the kernel's index and phase arithmetic
+    (gemm_bnstats_logic.h). Ring wrap-around across tiles, stage release one k-block behind, ragged M, both tile widths, the
+    swizzled staging layout, column sums merged over the two warpgroups and partial rows are checked against a plain GEMM."""
     r = subprocess.run(["make", "test_gemm_model"], cwd=REPO, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0 and "gemm_pipeline_model: all cases match" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
     assert "MISMATCH" not in r.stdout

@@ -202,23 +202,18 @@ def test_auth_token_file_protects_the_object_api(tmp_path, monkeypatch):
         op.stop()
 
 
-def test_models_match_the_reference_sdk_when_installed():
-    """Parity against the UNMODIFIED reference SDK installed at baseline/_ref (pip --target of
-    /root/reference/sdk/python/v2beta1): same openapi_types and attribute_map for all 9 MPIJob models."""
+def _reference_sdk_golden():
+    """What the UNMODIFIED reference SDK (sdk/python/v2beta1 of the reference) reports about its models, stored by
+    tests/golden/make_reference_sdk_golden.py."""
     import os
-    import subprocess
-    import sys
-    ref = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
-    if not os.path.isdir(os.path.join(ref, "mpijob")):
-        pytest.skip("reference SDK not installed (baseline/_ref)")
-    code = ("import sys, json; sys.path.insert(0, %r)\n"
-            "import mpijob.models as m\n"
-            "names = [n for n in dir(m) if n.startswith('V2beta1')]\n"
-            "print(json.dumps({n: [getattr(m, n).openapi_types, getattr(m, n).attribute_map] for n in names}))\n") % ref
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd="/tmp")
-    if r.returncode != 0:
-        pytest.skip("reference SDK not importable here: " + r.stderr[-200:])
-    theirs = json.loads(r.stdout)
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_sdk_models.json")) as f:
+        return json.load(f)
+
+
+def test_models_match_the_reference_sdk_when_installed():
+    """Parity against the reference SDK: same openapi_types and attribute_map for all 9 MPIJob models."""
+    theirs = _reference_sdk_golden()["v2beta1"]
+    assert len(theirs) == 9
     assert sorted(theirs) == sorted(n for n in mpijob.models.MODEL_CLASSES if n.startswith("V2beta1"))
     for name, (types, amap) in theirs.items():
         ours = mpijob.models.MODEL_CLASSES[name]
@@ -232,39 +227,9 @@ def test_models_match_the_reference_sdk_when_installed():
 
 def test_generic_models_match_the_reference_sdk_when_installed():
     """The 100 generic apimachinery models (sdk/meta_models.py, one schema table) against the generated files of the
-    UNMODIFIED reference SDK at baseline/_ref: same class names, module names, attribute maps and required fields."""
-    import os
-    import subprocess
-    import sys
+    reference SDK: same class names, module names, attribute maps and required fields."""
     from mpi_operator_b200.sdk.meta_models import snake
-    ref = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
-    if not os.path.isdir(os.path.join(ref, "mpijob")):
-        pytest.skip("reference SDK not installed (baseline/_ref)")
-    code = ("import sys, json, inspect; sys.path.insert(0, %r)\n"
-            "import mpijob.models as m\n"
-            "import importlib, pkgutil\n"
-            "out = {}\n"
-            "for info in pkgutil.iter_modules(m.__path__):            # every generated FILE (the package __init__ lists only half)\n"
-            "    mod = importlib.import_module('mpijob.models.' + info.name)\n"
-            "    cs = [c for c in vars(mod).values() if inspect.isclass(c) and c.__module__ == mod.__name__ and hasattr(c, 'attribute_map')]\n"
-            "    if len(cs) != 1 or cs[0].__name__.startswith('V2beta1'):\n"
-            "        continue\n"
-            "    c, n = cs[0], cs[0].__name__\n"
-            "    req = []\n"
-            "    for a in c.openapi_types:\n"
-            "        try:\n"
-            "            o = c.__new__(c); o.local_vars_configuration = type('C', (), {'client_side_validation': True})()\n"
-            "            setattr(o, a, None)\n"
-            "        except ValueError:\n"
-            "            req.append(a)\n"
-            "        except Exception:\n"
-            "            pass\n"
-            "    out[n] = [c.attribute_map, sorted(req), c.__module__.rsplit('.', 1)[-1]]\n"
-            "print(json.dumps(out))\n") % ref
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd="/tmp")
-    if r.returncode != 0:
-        pytest.skip("reference SDK not importable here: " + r.stderr[-200:])
-    theirs = json.loads(r.stdout)
+    theirs = _reference_sdk_golden()["generic"]
     assert len(theirs) == 100
     for name, (amap, required, module) in theirs.items():
         ours = mpijob.models.MODEL_CLASSES.get(name)
@@ -272,60 +237,6 @@ def test_generic_models_match_the_reference_sdk_when_installed():
         assert snake(name) == module, name
         assert set(amap.items()) <= set(ours.attribute_map.items()), name      # (the pod-template side may carry more fields)
         assert sorted(ours.required) == required, name
-
-
-def test_reference_sdk_example_runs_unmodified_through_the_kubernetes_shim(tmp_path):
-    """The reference's own SDK example (sdk/python/v2beta1/tensorflow-mnist.py: kubernetes.client models, the stale
-    `mpijob.V1ReplicaSpec` import, `config.load_kube_config()`, `CustomObjectsApi().create_namespaced_custom_object`) is
-    executed as is against the single-box daemon through the in-tree `kubernetes` compatibility package."""
-    import socket
-    import subprocess
-    import sys
-    ref = "/root/reference/sdk/python/v2beta1/tensorflow-mnist.py"
-    if not os.path.exists(ref):
-        pytest.skip("reference tree not mounted")
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
-    op = Operator(ServerOption(fake_gpus=2, leader_elect=False, state_dir=str(tmp_path)))
-    op.serve(f"127.0.0.1:{port}")
-    op.start()
-    try:
-        repo = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-        # run a byte-identical copy from an empty directory: next to the original lies the reference's own `mpijob` package,
-        # with which the example cannot even be imported (it no longer defines V1ReplicaSpec)
-        script = tmp_path / "tensorflow-mnist.py"
-        script.write_bytes(open(ref, "rb").read())
-        r = subprocess.run([sys.executable, str(script)], capture_output=True, text=True, timeout=60, cwd=str(tmp_path),
-                           env=dict(os.environ, PYTHONPATH=repo, MPIJOB_SERVER=f"127.0.0.1:{port}"))
-        assert r.returncode == 0, r.stdout + r.stderr
-        from kubernetes import client, config, watch
-        config.load_kube_config(host=f"127.0.0.1:{port}")
-        api = client.CustomObjectsApi()
-        job = api.get_namespaced_custom_object("kubeflow.org", "v2beta1", "default", "mpijobs", "tensorflow-mnist")
-        assert job["spec"]["mpiReplicaSpecs"]["Worker"]["replicas"] == 2 and job["spec"]["slotsPerWorker"] == 1
-        c = job["spec"]["mpiReplicaSpecs"]["Launcher"]["template"]["spec"]["containers"][0]
-        assert c["resources"] == {"limits": {"cpu": "1", "memory": "2Gi"}} and c["args"][:2] == ["-np", "2"]
-        # the example passes command="mpirun" (a string); the launcher pod the controller builds has the list form
-        launchers = [p for p in client.CoreV1Api().list_namespaced_pod("default", label_selector="training.kubeflow.org/job-role=launcher").items]
-        deadline = time.time() + 10
-        while not launchers and time.time() < deadline:
-            time.sleep(0.1)
-            launchers = client.CoreV1Api().list_namespaced_pod("default", label_selector="training.kubeflow.org/job-role=launcher").items
-        assert launchers and launchers[0].spec.containers[0].command == ["mpirun"] and launchers[0].metadata.name.startswith("tensorflow-mnist-launcher")
-        assert [j["metadata"]["name"] for j in api.list_namespaced_custom_object("kubeflow.org", "v2beta1", "default", "mpijobs")["items"]] == ["tensorflow-mnist"]
-        assert [j["metadata"]["name"] for j in api.list_cluster_custom_object("kubeflow.org", "v2beta1", "mpijobs")["items"]] == ["tensorflow-mnist"]
-        ev = next(iter(watch.Watch().stream(api.list_namespaced_custom_object, "kubeflow.org", "v2beta1", "default", "mpijobs", timeout_seconds=5)))
-        assert ev["type"] == "ADDED" and ev["object"]["metadata"]["name"] == "tensorflow-mnist"
-        api.patch_namespaced_custom_object("kubeflow.org", "v2beta1", "default", "mpijobs", "tensorflow-mnist", {"spec": {"runPolicy": {"suspend": True}}})
-        assert api.get_namespaced_custom_object_status("kubeflow.org", "v2beta1", "default", "mpijobs", "tensorflow-mnist")["spec"]["runPolicy"]["suspend"] is True
-        with pytest.raises(client.rest.ApiException):
-            api.get_namespaced_custom_object("example.com", "v1", "default", "widgets", "x")
-        core = client.CoreV1Api()
-        assert isinstance(core.list_namespaced_pod("default").items, list)
-        api.delete_namespaced_custom_object("kubeflow.org", "v2beta1", "default", "mpijobs", "tensorflow-mnist")
-        with pytest.raises(client.rest.ApiException):
-            api.get_namespaced_custom_object("kubeflow.org", "v2beta1", "default", "mpijobs", "tensorflow-mnist")
-    finally:
-        op.stop()
 
 
 def test_watch_stream_delivers_added_modified_deleted_in_order(tmp_path):

@@ -1,6 +1,6 @@
-"""tcgen05 GEMM + fused BN statistics (csrc/kernels/gemm_bnstats.cu) against a plain PyTorch fp32 reference.
+"""wgmma GEMM + fused BN statistics (csrc/kernels/gemm_bnstats.cu) against a plain PyTorch fp32 reference.
 
-First run on a B200 in round 2 (profiles/r2/session1_1gpu.log: 10 passed). Each case runs in a subprocess so that a trap in
+Each case runs in a subprocess so that a trap in
 the kernel (every wait is bounded and traps) cannot poison the CUDA context of the test session; the file sorts last for the
 same reason. B200MPI_SKIP_GEMM_TESTS=1 skips the file."""
 import os

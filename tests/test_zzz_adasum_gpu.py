@@ -1,14 +1,13 @@
 """Numerics of the one-kernel Adasum allreduce (csrc/kernels/adasum.cu) against the plain PyTorch fp32 tree
 (mpi_operator_b200/hvd/adasum.py: adasum_tree), on the emulated communicator (world virtual ranks on one GPU, the real
-multi-rank kernel with gridDim.y == world). The file sorts last in the GPU tier on purpose: the kernel was written after
-the round's GPU budget was spent, so its first execution is the driver's run; a failure here cannot mask another test.
+multi-rank kernel with gridDim.y == world). The file sorts last in the GPU tier on purpose: a fault in this kernel cannot
+mask another test.
 
 Reference call site: op=hvd.Adasum of examples/v2beta1/horovod/tensorflow_mnist.py:126-133 (SURVEY.md section 2.5, K6)."""
 import pytest
 import torch
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.xfail(strict=False, reason="k_adasum has not run on a B200 yet (written after the GPU budget was spent)")]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module", params=[2, 4, 8])

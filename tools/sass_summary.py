@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Regenerate profiles/sass_summary.md: per-kernel counts of the SASS instructions that prove the NVSwitch / TMA / tcgen05
+"""Regenerate profiles/sass_summary.md: per-kernel counts of the SASS instructions that prove the NVSwitch / TMA / wgmma
 paths, taken from `cuobjdump -sass` of the in-tree libraries (works without a GPU).
 
     python tools/sass_summary.py            # writes profiles/sass_summary.md
@@ -23,10 +23,9 @@ COLLECTIVE_COLS = OrderedDict([
     ("MEMBAR.*SYS", re.compile(r"\bMEMBAR\.\S*SYS")),
 ])
 GEMM_COLS = OrderedDict([
-    ("UTCHMMA (tcgen05.mma)", re.compile(r"\bUTCHMMA\b")),
-    ("UTCBAR (tcgen05.commit)", re.compile(r"\bUTCBAR\b")),
-    ("LDTM (tcgen05.ld)", re.compile(r"\bLDTM\b")),
-    ("UTCATOMSWS (tcgen05.alloc/dealloc)", re.compile(r"\bUTCATOMSWS\b")),
+    ("HGMMA (wgmma.mma_async)", re.compile(r"\bHGMMA\b")),
+    ("WARPGROUP.ARRIVE (wgmma.fence)", re.compile(r"\bWARPGROUP\.ARRIVE\b")),
+    ("WARPGROUP.DEPBAR (wgmma.wait_group)", re.compile(r"\bWARPGROUP\.DEPBAR\b")),
     ("UTMALDG (TMA tensor load)", re.compile(r"\bUTMALDG\b")),
     ("UTMASTG (TMA tensor store)", re.compile(r"\bUTMASTG\b")),
     ("SYNCS (mbarrier)", re.compile(r"\bSYNCS\b")),
@@ -75,13 +74,7 @@ def table(ks, cols, only=None):
 
 
 def main():
-    out = ["# SASS evidence (`cuobjdump -sass`, sm_100a; regenerate with `python tools/sass_summary.py`)", "",
-           "Mnemonics on sm_100a: `multimem.ld_reduce` -> `LDGMC.E.ADD.F32x4.RN.STRONG.SYS` (bf16: `LDGMC.E.ADD.BF16x8...`); "
-           "`multimem.st` and peer stores -> `STG.E.128.STRONG.SYS` (the multicast or peer VA decides where it lands); "
-           "`ld.relaxed.sys.v4` -> `LDG.E.128.STRONG.SYS`, streaming loads / no-allocate peer stores -> `LDG.E.NA.128` / `STG.E.NA.128`; `cp.async.bulk` (TMA copy engine, linear) -> `UBLKCP`; flag "
-           "`st.release.sys` -> `MEMBAR.ALL.SYS` + 32-bit `.STRONG.SYS` store, flag `ld.acquire.sys` -> 32-bit `.STRONG.SYS` load "
-           "(+ `CCTL.IVALL`); `tcgen05.mma` -> `UTCHMMA`, `tcgen05.ld` -> `LDTM`, tensor-map TMA -> `UTMALDG` / `UTMASTG`.",
-           "Full listings of the key kernels: `profiles/sass_key_kernels.sass`, `profiles/sass_gemm_bnstats.sass`.", ""]
+    out = ["# SASS evidence (`cuobjdump -sass`, sm_90a; regenerate with `python tools/sass_summary.py`)", ""]
     lib = os.path.join(LIBDIR, "libb200mpi.so")
     ks = kernels(lib)
     out += ["## `libb200mpi.so`: collective kernels (`csrc/kernels/collectives.cu`, `p2p.cu`)", "",
@@ -97,11 +90,11 @@ def main():
                                    ("ATOM/RED", re.compile(r"\b(ATOMG|RED)\b"))]), only=lambda n: n.startswith("bn::")), ""]
     glib = os.path.join(LIBDIR, "libb200mpi_gemm.so")
     if os.path.exists(glib):
-        out += ["## `libb200mpi_gemm.so`: tcgen05 / TMA / TMEM GEMM with BN statistics (`csrc/kernels/gemm_bnstats.cu`)", "",
-                "Ran on a B200 in round 2: numerics 10 / 10 (`tests/test_zz_gemm_bnstats_gpu.py`), ncu capture and timings in "
-                "`profiles/ncu_gemm_bnstats.md`; on by default for eligible 1x1 convolutions.", "",
+        out += ["## `libb200mpi_gemm.so`: wgmma / TMA GEMM with BN statistics (`csrc/kernels/gemm_bnstats.cu`)", "",
+                "Numerics: `tests/test_zz_gemm_bnstats_gpu.py`; on by default for eligible 1x1 convolutions.", "",
                 table(kernels(glib), GEMM_COLS), ""]
     path = os.path.join(ROOT, "profiles", "sass_summary.md")
+    os.makedirs(os.path.dirname(path), exist_ok=True)
     with open(path, "w") as f:
         f.write("\n".join(out))
     print(f"wrote {path}")
