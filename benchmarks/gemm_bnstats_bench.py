@@ -25,6 +25,19 @@ SHAPES = [(64 * 56 * 56, 64, 64), (64 * 56 * 56, 64, 256), (64 * 56 * 56, 256, 6
           (64 * 7 * 7, 1024, 512), (64 * 7 * 7, 512, 2048), (64 * 7 * 7, 2048, 512)]
 
 
+# conv1 data gradients of ResNet-101's residual blocks without downsample, with the residual gradient added in the epilogue:
+# (M, K = planes, N = 4 * planes, blocks per step)
+DGRAD_SHAPES = [(64 * 56 * 56, 64, 256, 2), (64 * 28 * 28, 128, 512, 3), (64 * 14 * 14, 256, 1024, 22), (64 * 7 * 7, 512, 2048, 2)]
+
+
+def dgrad_bytes_removed(m: int, n: int) -> int:
+    """HBM bytes per block that the residual epilogue removes. Before: bn3's backward writes dres = mask ⊙ dv (T), the
+    library dgrad writes its output (T), autograd's add reads both and writes the sum (3T). After: the kernel reads dv (T)
+    and the mask (T/16) and writes the sum (T). T = one bf16 [M, N] tensor."""
+    t = 2 * m * n
+    return 5 * t - (2 * t + t // 16)
+
+
 def timeit(fn, flush, iters):
     for _ in range(3):
         fn()
@@ -79,8 +92,29 @@ def main():
                      "ours_gbs": round(nbytes / t_ours / 1e6, 1), "ours_frac_hbm": round(nbytes / t_ours / 1e6 / peaks["hbm_gbs"], 3),
                      "ours_tflops": round(flops / t_ours / 1e9, 1), "ours_frac_bf16_peak": round(flops / t_ours / 1e9 / peaks["bf16_tflops"], 3)})
         print(json.dumps(rows[-1]), flush=True)
+    dgrad_rows, removed = [], 0
+    for m, k, n, blocks in DGRAD_SHAPES:
+        dy = torch.randn(m, k, device=dev, dtype=torch.bfloat16)
+        w2d = torch.randn(k, n, device=dev, dtype=torch.bfloat16) * (k ** -0.5)     # conv1 weight [Cout = planes, Cin]
+        dv = torch.randn(m, n, device=dev, dtype=torch.bfloat16)
+        mask = torch.randint(0, 256, (m * n // 8,), dtype=torch.uint8, device=dev)
+        dres = torch.randn(m, n, device=dev, dtype=torch.bfloat16)
+
+        def ours_dgrad():      # includes the per-step transposed copy of the weight
+            return gemm_bnstats.dgrad_residual(dy, w2d.t().contiguous(), dv, mask)
+
+        def library_dgrad():   # cuBLAS dgrad + autograd's add of the residual gradient bn3's backward wrote
+            return (dy @ w2d) + dres
+        t_ours, t_lib = timeit(ours_dgrad, flush, a.iters), timeit(library_dgrad, flush, a.iters)
+        removed += blocks * dgrad_bytes_removed(m, n)
+        nbytes = 2 * (m * k + k * n + 2 * m * n) + m * n // 8
+        dgrad_rows.append({"M": m, "K": k, "N": n, "blocks": blocks, "ours_us": round(1e3 * t_ours, 1),
+                           "cublas_dgrad_plus_add_us": round(1e3 * t_lib, 1), "speedup": round(t_lib / t_ours, 2),
+                           "ours_gbs": round(nbytes / t_ours / 1e6, 1), "step_bytes_removed": blocks * dgrad_bytes_removed(m, n)})
+        print(json.dumps(dgrad_rows[-1]), flush=True)
+    print(json.dumps({"dgrad_residual_bytes_removed_per_step": removed}), flush=True)
     out = {"peaks": {k_: peaks[k_] for k_ in ("hbm_gbs", "bf16_tflops")}, "l2": "256 MiB buffer rewritten between iterations",
-           "iters": a.iters, "rows": rows}
+           "iters": a.iters, "rows": rows, "dgrad_rows": dgrad_rows, "dgrad_residual_bytes_removed_per_step": removed}
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:

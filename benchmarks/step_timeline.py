@@ -58,6 +58,63 @@ def subtract(iv, mask):
     return out
 
 
+KERNEL_CLASSES = ("bn_fwd", "bn_reduce", "bn_finalize", "bn_elemt", "autograd_add", "cublas_dgrad", "cublas_wgrad", "cudnn",
+                  "wgmma_gemm", "weight_copy", "memset", "other")
+
+
+def kernel_class(name: str, op: str, dims) -> str:
+    """Device-time class of one kernel record. `op` / `dims` are the innermost CPU op that launched it and that op's input
+    shapes (record_shapes): they tell autograd's gradient add from other elementwise kernels, and a 1x1 dgrad GEMM
+    (dy [M,Cout] @ w [Cout,Cin]: inner dimension = a channel count) from its wgrad (dy^T @ x: inner dimension = M). That
+    split assumes M > 2048, the widest ResNet channel count: true at batch 64, not for the 7x7 stage below batch 42.
+    weight_copy: 2-D copies, i.e. the per-step transposed 1x1 weights the wgmma dgrad reads."""
+    if "k_gemm_bnstats" in name or "k_gemm_dgrad" in name:
+        return "wgmma_gemm"
+    if "k_bn_bwd_reduce" in name:
+        return "bn_reduce"
+    if "finalize" in name and "k_bn_" in name:
+        return "bn_finalize"
+    if "k_bn_bwd_elemt" in name:
+        return "bn_elemt"
+    if "k_bn_fwd" in name:
+        return "bn_fwd"
+    if op in ("aten::copy_", "aten::clone", "aten::contiguous") and dims and len(dims[0] or ()) == 2:
+        return "weight_copy"
+    if op in ("aten::add", "aten::add_") and "elementwise" in name:
+        return "autograd_add"
+    if op in ("aten::mm", "aten::addmm", "aten::matmul"):
+        try:
+            inner = int(dims[0][1])
+        except (TypeError, ValueError, IndexError):
+            inner = 0
+        return "cublas_wgrad" if inner > 2048 else "cublas_dgrad"   # every ResNet channel count is <= 2048 < M
+    if op.startswith("aten::cudnn") or op.startswith("aten::convolution") or "cudnn" in name:
+        return "cudnn"
+    return "other"
+
+
+def class_breakdown(trace: dict, steps: int) -> dict:
+    """Device time (us) and kernel count per step for every KERNEL_CLASSES entry."""
+    ops, corr_ext = {}, {}
+    for e in trace["traceEvents"]:
+        a = e.get("args") or {}
+        if e.get("cat") == "cpu_op" and "External id" in a:
+            ops[a["External id"]] = (e.get("name", ""), a.get("Input Dims"))
+        elif e.get("cat") == "cuda_runtime" and "correlation" in a and "External id" in a:
+            corr_ext[a["correlation"]] = a["External id"]
+    out = {c: {"us": 0.0, "kernels": 0} for c in KERNEL_CLASSES}
+    for e in trace["traceEvents"]:
+        if e.get("cat") not in ("kernel", "gpu_memset") or "dur" not in e:
+            continue
+        a = e.get("args") or {}
+        ext = a.get("External id", corr_ext.get(a.get("correlation")))
+        op, dims = ops.get(ext, ("", None))
+        c = "memset" if e["cat"] == "gpu_memset" else kernel_class(e["name"], op, dims)
+        out[c]["us"] += e["dur"] / steps
+        out[c]["kernels"] += 1 / steps
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=3)
@@ -80,15 +137,16 @@ def main():
     torch.cuda.synchronize()
     comm.host_barrier()
     from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
+    with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU], record_shapes=True) as prof:
         for i in range(a.steps):
             tr.step(xs[i % 2], ys[i % 2])
         torch.cuda.synchronize()
     comm.host_barrier()
     path = f"/tmp/b200mpi_timeline_{os.getpid()}.json"
     prof.export_chrome_trace(path)
-    ev = [e for e in json.load(open(path))["traceEvents"] if e.get("cat") in ("kernel", "gpu_memcpy", "gpu_memset") and "dur" in e]
+    trace = json.load(open(path))
     os.unlink(path)
+    ev = [e for e in trace["traceEvents"] if e.get("cat") in ("kernel", "gpu_memcpy", "gpu_memset") and "dur" in e]
     comm_k = [e for e in ev if "k_allreduce" in e["name"] or "b200mpi::k_" in e["name"]]
     comm_streams = {e["args"].get("stream") for e in comm_k}
     h2d = [e for e in ev if e.get("cat") == "gpu_memcpy" and "HtoD" in e["name"]]
@@ -118,6 +176,7 @@ def main():
         last_comp_end = max((e["ts"] + e["dur"] for e in before), default=last["ts"])
         tails.append({"name": last["name"][:60], "dur_us": last["dur"], "exposed_us": max(0.0, last["ts"] + last["dur"] - max(last_comp_end, last["ts"]))})
     rep["tail_bucket"] = tails
+    rep["classes"] = class_breakdown(trace, a.steps)
     import struct
     blob = json.dumps(rep).encode()
     if world > 1:
@@ -128,7 +187,11 @@ def main():
         for k in ("span_us_per_step", "compute_busy_us", "comm_busy_us", "comm_exposed_us", "h2d_busy_us", "h2d_exposed_us"):
             lines.append(f"| {k} | {rep[k]:.0f} |")
         lines += ["", f"comm kernels per step: {rep['comm_kernels_per_step']:.0f}; H2D on the compute stream: {rep['h2d_stream_is_compute_stream']}", "",
-                  "tail bucket (last comm kernel of each step): " + json.dumps(tails), ""]
+                  "tail bucket (last comm kernel of each step): " + json.dumps(tails), "",
+                  "| kernel class | device us / step | kernels / step |", "|---|---|---|"]
+        for c, v in rep["classes"].items():
+            lines.append(f"| {c} | {v['us']:.0f} | {v['kernels']:.0f} |")
+        lines.append("")
         text = "\n".join(lines)
         print(text)
         print("JSON " + json.dumps(rep))

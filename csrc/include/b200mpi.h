@@ -217,6 +217,11 @@ int b200mpi_bn_act_bwd(const void* dz, const void* x, const void* mask, void* dx
                        const float* weight, const float* save_mean, const float* save_invstd,
                        float* dweight, float* dbias, float* workspace, long long M, int C, int relu,
                        void* stream);
+/* Same as b200mpi_bn_act_bwd but the reduction arrives as `parts` rows of {sum g, sum g*(x - save_mean)} (g = mask ⊙ dz,
+ * 2*C floats per row) produced by the epilogue of the wgmma dgrad: no reduce pass over dz. */
+int b200mpi_bn_act_bwd_prestats(const void* dz, const void* x, const void* mask, void* dx, void* dres, const float* weight,
+                                const float* save_mean, const float* save_invstd, float* dweight, float* dbias, float* workspace,
+                                const float* partials, int parts, long long M, int C, int relu, void* stream);
 
 /* tuning */
 int b200mpi_set_tuning(b200mpi_comm_t comm, size_t oneshot_max_bytes, size_t nvls_min_bytes,

@@ -432,6 +432,31 @@ int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, vo
   return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
 }
 
+static void bwd_elemt(const void* dz, const void* x, const void* mask, void* dx, void* dres, const float* coef, long long M, int C,
+                      int relu, cudaStream_t s) {
+  int grid;
+  long long rows;
+  plan(M, C, 1184, (dres ? 8LL : 6LL) * C, &grid, &rows, elem_chunk());
+  if (relu && dres) k_bn_bwd_elemt<true, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, (const uint8_t*)mask, (uint4*)dx, (uint4*)dres, coef, M, C, rows);
+  else if (relu) k_bn_bwd_elemt<true, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, (const uint8_t*)mask, (uint4*)dx, nullptr, coef, M, C, rows);
+  else if (dres) k_bn_bwd_elemt<false, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, nullptr, (uint4*)dx, (uint4*)dres, coef, M, C, rows);
+  else k_bn_bwd_elemt<false, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, nullptr, (uint4*)dx, nullptr, coef, M, C, rows);
+}
+
+// Backward with the reduction already done: `parts` rows of per-channel {sum g, sum g * (x - save_mean)} (g = mask ⊙ dz)
+// taken by the producer of dz — the epilogue of the wgmma dgrad (gemm_bnstats.cu). Finalize + elemt only: the reduce
+// pass over dz, x and the mask is gone. dres == nullptr skips the residual-gradient write.
+int b200mpi_bn_act_bwd_prestats(const void* dz, const void* x, const void* mask, void* dx, void* dres, const float* weight,
+                                const float* save_mean, const float* save_invstd, float* dweight, float* dbias, float* workspace,
+                                const float* partials, int parts, long long M, int C, int relu, void* stream_) {
+  if (!b200mpi_bn_supported(M, C) || parts < 1 || !partials) return B200MPI_ERR_UNSUPPORTED;
+  cudaStream_t s = (cudaStream_t)stream_;
+  float* coef = workspace;
+  k_bn_bwd_finalize<<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>(partials, parts, coef, M, C, weight, save_mean, save_invstd, dweight, dbias);
+  bwd_elemt(dz, x, mask, dx, dres, coef, M, C, relu, s);
+  return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
+}
+
 int b200mpi_bn_act_bwd(const void* dz, const void* x, const void* mask, void* dx, void* dres, const float* weight,
                        const float* save_mean, const float* save_invstd, float* dweight, float* dbias, float* workspace,
                        long long M, int C, int relu, void* stream_) {
@@ -445,11 +470,7 @@ int b200mpi_bn_act_bwd(const void* dz, const void* x, const void* mask, void* dx
   if (relu) k_bn_bwd_reduce<true><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, (const uint8_t*)mask, partials, M, C, rows, save_mean);
   else k_bn_bwd_reduce<false><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, nullptr, partials, M, C, rows, save_mean);
   k_bn_bwd_finalize<<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>(partials, grid, coef, M, C, weight, save_mean, save_invstd, dweight, dbias);
-  plan(M, C, 1184, (dres ? 8LL : 6LL) * C, &grid, &rows, elem_chunk());
-  if (relu && dres) k_bn_bwd_elemt<true, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, (const uint8_t*)mask, (uint4*)dx, (uint4*)dres, coef, M, C, rows);
-  else if (relu) k_bn_bwd_elemt<true, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, (const uint8_t*)mask, (uint4*)dx, nullptr, coef, M, C, rows);
-  else if (dres) k_bn_bwd_elemt<false, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, nullptr, (uint4*)dx, (uint4*)dres, coef, M, C, rows);
-  else k_bn_bwd_elemt<false, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)dz, (const uint4*)x, nullptr, (uint4*)dx, nullptr, coef, M, C, rows);
+  bwd_elemt(dz, x, mask, dx, dres, coef, M, C, relu, s);
   return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
 }
 

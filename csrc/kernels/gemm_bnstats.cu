@@ -6,6 +6,10 @@
 //   partials[p][2n+0] += sum_m Y[m,n],  partials[p][2n+1] += sum_m Y[m,n]^2      (one row per CTA m-group, the layout the
 //                                                                                  BN finalize kernel of bn_act.cu merges)
 //
+// The same kernel with RES = true is the data gradient of a residual block's first 1x1 convolution (b200mpi_gemm_dgrad_res):
+//   dX[M,N] = dY[M,K] . Wt[N,K]^T + mask ⊙ R    (R = gradient of the block output, mask = its 1-bit ReLU mask; no statistics)
+// so that the residual gradient never exists as a tensor of its own and autograd adds nothing.
+//
 // Why: two thirds of ResNet's BatchNorm layers follow a 1x1 convolution. Their statistics pass re-reads the whole
 // convolution output from HBM; here the tile is still in shared memory when its column sums are taken, so the pass
 // disappears. The reference has no kernels at all (SURVEY.md §2.2) — this is part of the data plane the new framework adds.
@@ -148,33 +152,53 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-template <int BN>
+// RES = the dgrad epilogue: out = acc + mask ⊙ R (R a bf16 [M,N] tensor, mask its 1-bit ReLU mask).
+// GST (needs RES) = also the BN-backward partials of the BatchNorm whose output the convolution read: per column
+// sum g and sum g * (Xb - mean_b), g = maskB ⊙ bf16(out), Xb = that BN's saved input, maskB its ReLU mask; one row per CTA
+// in the layout k_bn_bwd_finalize merges (instead of the forward's sum / sum of squares).
+// The epilogue operands are TMA-loaded by the producer into a region of their own while the tile's last k-blocks run; with
+// GST the operand ring has 3 stages so that everything fits in shared memory.
+template <int BN, bool RES, bool GST>
 struct Smem {
+  static constexpr int kS = GST ? 3 : kStages;
   static constexpr uint32_t kBBytes = BN * BK * 2;
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kOutBoxes = BN / 64;                  // TMA store boxes of [128 rows x 64 cols] (128 B inner)
   static constexpr uint32_t kOutBytes = kOutBoxes * kBoxBytes;
+  static constexpr uint32_t kResBytes = RES ? kOutBytes : 0;      // residual tile, same swizzled layout as the staging
+  static constexpr uint32_t kMaskBytes = RES ? BM * BN / 8 : 0;
+  static constexpr uint32_t kXbBytes = GST ? kOutBytes : 0;       // the lower BN's input tile, same layout
+  static constexpr uint32_t kMaskBBytes = GST ? BM * BN / 8 : 0;
   static constexpr uint32_t kA = 0;
-  static constexpr uint32_t kB = kStages * kABytes;
-  static constexpr uint32_t kOut = kB + kStages * kBBytes;
-  static constexpr uint32_t kSums = kOut + kOutBytes;             // [BN][2] fp32: warpgroup 1's column sums
-  static constexpr uint32_t kBars = kSums + BN * 8;               // full[S], empty[S]
-  static constexpr uint32_t kTotal = kBars + 2 * kStages * 8;
+  static constexpr uint32_t kB = kS * kABytes;
+  static constexpr uint32_t kOut = kB + kS * kBBytes;
+  static constexpr uint32_t kRes = kOut + kOutBytes;
+  static constexpr uint32_t kMask = kRes + kResBytes;
+  static constexpr uint32_t kXb = kMask + kMaskBytes;             // 1024-aligned: kMaskBytes is a multiple of 1024 for BN=128
+  static constexpr uint32_t kMaskB = kXb + kXbBytes;
+  static constexpr uint32_t kSums = kMaskB + kMaskBBytes;         // [BN][2] fp32: warpgroup 1's column sums
+  static constexpr uint32_t kBars = kSums + BN * 8;               // full[S], empty[S], res_full, res_empty
+  static constexpr uint32_t kTotal = kBars + (2 * kS + 2) * 8;
   static constexpr uint32_t kDynamic = kTotal + 1024;             // slack to align the base to 1024 B (swizzle atoms)
 };
 
-template <int BN>
+template <int BN, bool RES, bool GST>
 __global__ void __launch_bounds__(kThreads, 1)
 k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmY,
+               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmMask,
+               const __grid_constant__ CUtensorMap tmXb, const __grid_constant__ CUtensorMap tmMaskB, const float* __restrict__ mean_b,
                float* __restrict__ partials, int M, int N, int K, int num_n) {
-  using L = Smem<BN>;
+  using L = Smem<BN, RES, GST>;
+  constexpr int S = L::kS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t sA = base + L::kA, sB = base + L::kB, sOut = base + L::kOut, sBar = base + L::kBars;
+  const uint32_t sRes = base + L::kRes, sMask = base + L::kMask, sXb = base + L::kXb, sMaskB = base + L::kMaskB;
   float* sums = reinterpret_cast<float*>(base_ptr + L::kSums);
   auto full_bar = [&](int s) { return sBar + 8u * s; };
-  auto empty_bar = [&](int s) { return sBar + 8u * (kStages + s); };
+  auto empty_bar = [&](int s) { return sBar + 8u * (S + s); };
+  const uint32_t res_full = sBar + 8u * (2 * S), res_empty = res_full + 8u;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const TileWalk walk((int)blockIdx.x, (int)gridDim.x, num_n, M);
@@ -186,9 +210,19 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
     tma_prefetch_desc(&tmY);
-    for (int s = 0; s < kStages; s++) {
+    for (int s = 0; s < S; s++) {
       mbar_init(full_bar(s), 1);                   // producer's arrive.expect_tx (+ the TMA transaction bytes)
       mbar_init(empty_bar(s), kConsumers / 32);    // one arrive per consumer warp once its wgmma has read the stage
+    }
+    if (RES) {
+      tma_prefetch_desc(&tmR);
+      tma_prefetch_desc(&tmMask);
+      mbar_init(res_full, 1);
+      mbar_init(res_empty, kConsumers / 32);       // one arrive per consumer warp once it has read the epilogue operands
+    }
+    if (GST) {
+      tma_prefetch_desc(&tmXb);
+      tma_prefetch_desc(&tmMaskB);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -198,14 +232,28 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   if (warp == kConsumers / 32) {
     // ===================================================== TMA producer ====
     if (lane == 0) {
-      Ring st;
+      Ring st, rs;
       for (int m_blk = m_first; m_blk < num_m; m_blk += m_step) {
         for (int kb = 0; kb < num_k; kb++) {
           mbar_wait(empty_bar(st.s), st.ph ^ 1u);
           mbar_arrive_expect_tx(full_bar(st.s), L::kStageBytes);
           tma_load_2d(sA + st.s * kABytes, &tmX, full_bar(st.s), kb * BK, m_blk * BM);
           tma_load_2d(sB + st.s * L::kBBytes, &tmW, full_bar(st.s), kb * BK, n0);
-          st.advance(kStages);
+          st.advance(S);
+        }
+        if (RES) {
+          // the tile's operands are all in flight: fetch its epilogue operands once the previous tile's epilogue has read them
+          mbar_wait(res_empty, rs.ph ^ 1u);
+          mbar_arrive_expect_tx(res_full, L::kResBytes + L::kMaskBytes + L::kXbBytes + L::kMaskBBytes);
+#pragma unroll
+          for (int b = 0; b < (int)L::kOutBoxes; b++) tma_load_2d(sRes + (uint32_t)b * kBoxBytes, &tmR, res_full, n0 + b * 64, m_blk * BM);
+          tma_load_2d(sMask, &tmMask, res_full, n0 / 8, m_blk * BM);
+          if (GST) {
+#pragma unroll
+            for (int b = 0; b < (int)L::kOutBoxes; b++) tma_load_2d(sXb + (uint32_t)b * kBoxBytes, &tmXb, res_full, n0 + b * 64, m_blk * BM);
+            tma_load_2d(sMaskB, &tmMaskB, res_full, n0 / 8, m_blk * BM);
+          }
+          rs.advance(1);
         }
       }
     }
@@ -219,8 +267,9 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const bool col_owner = t < BN;
   const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   float s1 = 0.f, s2 = 0.f;
+  const float mu = (GST && col_owner) ? mean_b[n0 + t] : 0.f;
   float d[BN / 2] = {};
-  Ring st;
+  Ring st, rs;
   for (int m_blk = m_first; m_blk < num_m; m_blk += m_step) {
     int prev = 0;
     for (int kb = 0; kb < num_k; kb++) {
@@ -238,7 +287,7 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         if (lane == 0) mbar_arrive(empty_bar(prev));
       }
       prev = st.s;
-      st.advance(kStages);
+      st.advance(S);
     }
     wgmma_wait<0>();
     __syncwarp();
@@ -246,6 +295,28 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
 
     if (ct == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous tile's store has read the staging
     cons_bar_sync();                                                               // ... and its column sums are taken
+    if (RES) {
+      // out = acc + mask ⊙ R in fp32, rounded to bf16 once
+      mbar_wait(res_full, rs.ph);
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) {
+        const int col = 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+          uint32_t r2, mk;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r2) : "r"(sRes + stage_elem_byte(col, frag_row + 8 * i)) : "memory");
+          asm volatile("ld.shared.u8 %0, [%1];" : "=r"(mk) : "r"(sMask + mask_byte(BN, col, frag_row + 8 * i)) : "memory");
+          const uint32_t bits = mk >> (col & 7);
+          if (bits & 1u) d[4 * j + 2 * i] += __uint_as_float(r2 << 16);
+          if (bits & 2u) d[4 * j + 2 * i + 1] += __uint_as_float(r2 & 0xffff0000u);
+        }
+      }
+      if (!GST) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(res_empty);
+        rs.advance(1);
+      }
+    }
     // fp32 fragment -> bf16 pairs in the swizzled staging layout (gemm_bnstats_logic.h)
 #pragma unroll
     for (int j = 0; j < BN / 8; j++) {
@@ -264,7 +335,7 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       for (int b = 0; b < (int)L::kOutBoxes; b++) tma_store_2d(&tmY, sOut + (uint32_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
-    if (col_owner) {
+    if (!RES && col_owner) {
       // column sums of the bf16-rounded tile (what the BN apply pass will read back). Rows past M are zero-filled by TMA.
 #pragma unroll 8
       for (int r = wg * 64; r < wg * 64 + 64; r++) {
@@ -275,13 +346,33 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
         s2 = fmaf(f, f, s2);
       }
     }
+    if (GST) {
+      if (col_owner) {
+        // BN-backward partials of the lower layer from the bf16-rounded tile (what its elemt pass will read back as dz).
+        // Rows past M: TMA zero-fills the mask, so they add nothing.
+#pragma unroll 8
+        for (int r = wg * 64; r < wg * 64 + 64; r++) {
+          uint16_t h, xh;
+          uint32_t mk;
+          asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(sOut + stage_elem_byte(t, r)));
+          asm volatile("ld.shared.u16 %0, [%1];" : "=h"(xh) : "r"(sXb + stage_elem_byte(t, r)) : "memory");
+          asm volatile("ld.shared.u8 %0, [%1];" : "=r"(mk) : "r"(sMaskB + mask_byte(BN, t, r)) : "memory");
+          const float g = (mk >> (t & 7)) & 1u ? __uint_as_float((uint32_t)h << 16) : 0.f;
+          s1 += g;
+          s2 = fmaf(g, __uint_as_float((uint32_t)xh << 16) - mu, s2);
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(res_empty);
+      rs.advance(1);
+    }
   }
-  if (wg == 1 && col_owner) {
+  if ((!RES || GST) && wg == 1 && col_owner) {
     sums[2 * t] = s1;
     sums[2 * t + 1] = s2;
   }
   cons_bar_sync();
-  if (wg == 0 && col_owner && m_first < num_m) {
+  if ((!RES || GST) && wg == 0 && col_owner && m_first < num_m) {
     float* row_out = partials + partial_index(m_first, N, n0 + t);
     row_out[0] = s1 + sums[2 * t];
     row_out[1] = s2 + sums[2 * t + 1];
@@ -327,23 +418,54 @@ static int sm_count() {
   return n;
 }
 
-template <int BN>
-static int launch(const void* X, const void* W, void* Y, float* partials, int* parts_out, long long M, int N, int K, cudaStream_t s) {
-  CUtensorMap tmX, tmW, tmY;
+// row-major [rows, cols] uint8 matrix (a 1-bit-per-element mask, cols = elements / 8), box = [box_rows, box_cols], unswizzled
+static bool make_mask_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return false;
+  const cuuint64_t dims[2] = {cols, rows};
+  const cuuint64_t strides[1] = {cols};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  return fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// RES: R and mask are the residual operand of the dgrad epilogue; GST: Xb, maskB, mean_b are the lower BN's saved input,
+// ReLU mask and mean, and partials receive its backward partials; otherwise partials receive the column statistics.
+template <int BN, bool RES, bool GST>
+static int launch(const void* X, const void* W, void* Y, float* partials, int* parts_out, const void* R, const void* mask, const void* Xb,
+                  const void* maskB, const float* mean_b, long long M, int N, int K, cudaStream_t s) {
+  CUtensorMap tmX, tmW, tmY, tmR, tmMask, tmXb, tmMaskB;
   if (!make_map(&tmX, X, (uint64_t)M, (uint64_t)K, BM) || !make_map(&tmW, W, (uint64_t)N, (uint64_t)K, BN) ||
       !make_map(&tmY, Y, (uint64_t)M, (uint64_t)N, BM))
     return B200MPI_ERR_CUDA;
+  if (RES) {
+    if (!make_map(&tmR, R, (uint64_t)M, (uint64_t)N, BM) || !make_mask_map(&tmMask, mask, (uint64_t)M, (uint64_t)N / 8, BM, BN / 8))
+      return B200MPI_ERR_CUDA;
+  } else {
+    tmR = tmY;      // unused
+    tmMask = tmY;
+  }
+  if (GST) {
+    if (!make_map(&tmXb, Xb, (uint64_t)M, (uint64_t)N, BM) || !make_mask_map(&tmMaskB, maskB, (uint64_t)M, (uint64_t)N / 8, BM, BN / 8))
+      return B200MPI_ERR_CUDA;
+  } else {
+    tmXb = tmY;     // unused
+    tmMaskB = tmY;
+  }
   const int num_n = N / BN, num_m = (int)((M + BM - 1) / BM);
   int groups = (sm_count() < kMaxParts ? sm_count() : kMaxParts) / num_n;
   if (groups < 1) return B200MPI_ERR_UNSUPPORTED;
   if (groups > num_m) groups = num_m;
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(k_gemm_bnstats<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Smem<BN>::kDynamic) != cudaSuccess)
+    if (cudaFuncSetAttribute(k_gemm_bnstats<BN, RES, GST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)Smem<BN, RES, GST>::kDynamic) != cudaSuccess)
       return B200MPI_ERR_CUDA;
     attr_set = true;
   }
-  k_gemm_bnstats<BN><<<groups * num_n, kThreads, Smem<BN>::kDynamic, s>>>(tmX, tmW, tmY, partials, (int)M, N, K, num_n);
+  k_gemm_bnstats<BN, RES, GST><<<groups * num_n, kThreads, Smem<BN, RES, GST>::kDynamic, s>>>(tmX, tmW, tmY, tmR, tmMask, tmXb, tmMaskB,
+                                                                                              mean_b, partials, (int)M, N, K, num_n);
   if (parts_out) *parts_out = groups;
   return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
 }
@@ -369,7 +491,29 @@ int b200mpi_gemm_bnstats(const void* X, const void* W, void* Y, float* partials,
   if (!b200mpi_gemm_bnstats_supported(M, N, K)) return B200MPI_ERR_UNSUPPORTED;
   if (((uintptr_t)X | (uintptr_t)W | (uintptr_t)Y) & 15) return B200MPI_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
-  return N % 128 == 0 ? launch<128>(X, W, Y, partials, parts, M, N, K, s) : launch<64>(X, W, Y, partials, parts, M, N, K, s);
+  return N % 128 == 0 ? launch<128, false, false>(X, W, Y, partials, parts, nullptr, nullptr, nullptr, nullptr, nullptr, M, N, K, s)
+                      : launch<64, false, false>(X, W, Y, partials, parts, nullptr, nullptr, nullptr, nullptr, nullptr, M, N, K, s);
+}
+
+// Data gradient of a 1x1 convolution whose input also feeds a residual add followed by a ReLU:
+//   dX[M,N] = dY[M,K] . Wt[N,K]^T + mask ⊙ R      (Wt = the convolution weight transposed to [Cin, Cout]; R [M,N] bf16 =
+// the gradient of the block output, mask [M, N/8] = the 1-bit ReLU mask of that output), summed in fp32, rounded once.
+// With Xb != nullptr also the backward partials of the BatchNorm that produced the convolution's input (Xb [M,N] bf16 = its
+// saved input, maskB [M, N/8] = its ReLU mask, mean_b [N] = its saved mean): partials[parts][2N] = per column
+// {sum g, sum g * (Xb - mean_b)}, g = maskB ⊙ dX, the rows b200mpi_bn_act_bwd_prestats takes; *parts = rows written.
+int b200mpi_gemm_dgrad_res_supported(long long M, int N, int K) {
+  return (b200mpi_gemm_bnstats_supported(M, N, K) && N % 128 == 0) ? 1 : 0;
+}
+
+int b200mpi_gemm_dgrad_res(const void* dY, const void* Wt, void* dX, const void* R, const void* mask, const void* Xb, const void* maskB,
+                           const float* mean_b, float* partials, int* parts, long long M, int N, int K, void* stream) {
+  using namespace b200mpi::gemm;
+  if (!b200mpi_gemm_dgrad_res_supported(M, N, K)) return B200MPI_ERR_UNSUPPORTED;
+  if (((uintptr_t)dY | (uintptr_t)Wt | (uintptr_t)dX | (uintptr_t)R | (uintptr_t)mask | (uintptr_t)Xb | (uintptr_t)maskB) & 15)
+    return B200MPI_ERR_INVALID;
+  if (!Xb) return launch<128, true, false>(dY, Wt, dX, nullptr, parts, R, mask, nullptr, nullptr, nullptr, M, N, K, (cudaStream_t)stream);
+  if (!maskB || !mean_b || !partials) return B200MPI_ERR_INVALID;
+  return launch<128, true, true>(dY, Wt, dX, partials, parts, R, mask, Xb, maskB, mean_b, M, N, K, (cudaStream_t)stream);
 }
 
 }  // extern "C"

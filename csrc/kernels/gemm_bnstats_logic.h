@@ -53,6 +53,9 @@ B200_HD uint32_t stage_elem_byte(int col, int r) {
 B200_HD uint32_t operand_elem_byte(int r, int k) {
   return (uint32_t)r * 128u + ((((uint32_t)k >> 3) ^ (uint32_t)(r & 7)) << 4) + (uint32_t)(k & 7) * 2u;
 }
+// Residual-gradient epilogue (dgrad): the ReLU mask tile TMA loads next to the residual tile is [128 rows x BN/8 bytes],
+// unswizzled; bit (col & 7) of byte (row, col / 8) is the mask of tile element (row, col).
+B200_HD uint32_t mask_byte(int BN, int col, int r) { return (uint32_t)r * (uint32_t)(BN / 8) + (uint32_t)(col >> 3); }
 // partials[m_first][2 * global_column + {0: sum, 1: sum of squares}]
 B200_HD size_t partial_index(int m_first, int N, int global_col) { return (size_t)m_first * 2 * (size_t)N + 2 * (size_t)global_col; }
 

@@ -81,6 +81,9 @@ struct Problem {
   int M, N, K, BN;
   std::vector<uint16_t> X, W, Y;   // row-major bf16: X [M,K], W [N,K], Y [M,N]
   std::vector<float> partials;     // [parts][2N]
+  bool res = false;                // dgrad epilogue: Y = X.W^T + mask ⊙ R, no statistics
+  std::vector<uint16_t> R;         // [M,N] bf16
+  std::vector<uint8_t> mask;       // [M, N/8]: bit c%8 of byte c/8
 };
 
 // ------------------------------------------------------------------- CTA ----
@@ -91,15 +94,19 @@ struct CTA {
   const int cta, grid, num_n;
   const int BN;
   std::vector<uint8_t> sA, sB, sOut;                 // kStages x tile, kStages x tile, BN/64 boxes
+  std::vector<uint8_t> sRes, sMask;                  // residual tile (staging layout) and its mask tile
   std::vector<float> sums;                           // [BN][2]: warpgroup 1's column sums
   MBar full[kStages], empty[kStages];
+  MBar res_full, res_empty;
   NamedBarrier cons{2};                              // bar.sync 1, 256: the two consumer warpgroups (one thread each)
   std::mutex store_mu;                               // the TMA store "bulk group": finished when it returns
 
   CTA(Problem& p_, int cta_, int grid_, int num_n_)
       : p(p_), cta(cta_), grid(grid_), num_n(num_n_), BN(p_.BN), sA((size_t)kStages * BM * 128), sB((size_t)kStages * p_.BN * 128),
-        sOut((size_t)(p_.BN / 64) * kBoxBytes), sums((size_t)2 * p_.BN, 0.f) {
+        sOut((size_t)(p_.BN / 64) * kBoxBytes), sRes(sOut.size()), sMask((size_t)BM * p_.BN / 8), sums((size_t)2 * p_.BN, 0.f) {
     for (int s = 0; s < kStages; s++) { full[s].reset(1); empty[s].reset(kConsumerWarps); }
+    res_full.reset(1);
+    res_empty.reset(kConsumerWarps);
   }
 
   // cp.async.bulk.tensor.2d load with SWIZZLE_128B: box of `rows` x 64 elements at (row0, k0), zero fill outside the matrix
@@ -136,13 +143,24 @@ struct CTA {
         d[(size_t)m * BN + n] = acc;
       }
   }
+  // the residual tile ([128 x 64] SWIZZLE_128B boxes, zero fill past M) and its mask tile ([128 x BN/8] bytes, unswizzled)
+  void tma_load_res(int n0, int row0) {
+    for (int r = 0; r < BM; r++)
+      for (int c = 0; c < BN; c++) {
+        const bool in = row0 + r < p.M;
+        const uint16_t v = in ? p.R[(size_t)(row0 + r) * p.N + n0 + c] : 0;
+        memcpy(sRes.data() + stage_elem_byte(c, r), &v, 2);
+        if (c % 8 == 0) sMask[mask_byte(BN, c, r)] = in ? p.mask[(size_t)(row0 + r) * (p.N / 8) + (n0 + c) / 8] : 0;
+      }
+    res_full.complete_tx((long long)sRes.size() + (long long)sMask.size());
+  }
   void release(int s) { for (int w = 0; w < kConsumerWarps / 2; w++) empty[s].arrive(); }   // lane 0 of each warp
 
   void producer() {  // warp 8, lane 0
     const TileWalk walk(cta, grid, num_n, p.M);
     const int num_k = p.K / BK, n0 = walk.n_blk * BN;
-    Ring st;
-    for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step)
+    Ring st, rs;
+    for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step) {
       for (int kb = 0; kb < num_k; kb++) {
         empty[st.s].wait(st.ph ^ 1u);
         full[st.s].arrive_expect_tx((long long)BM * 128 + (long long)BN * 128);
@@ -150,6 +168,13 @@ struct CTA {
         tma_load(sB.data() + (size_t)st.s * BN * 128, p.W, p.N, n0, kb * BK, BN, full[st.s]);
         st.advance(kStages);
       }
+      if (p.res) {
+        res_empty.wait(rs.ph ^ 1u);
+        res_full.arrive_expect_tx((long long)sRes.size() + (long long)sMask.size());
+        tma_load_res(n0, m_blk * BM);
+        rs.advance(1);
+      }
+    }
   }
   // one consumer warpgroup; its 128 threads are executed one after the other between barriers
   void consumer(int wg) {
@@ -157,7 +182,7 @@ struct CTA {
     const int num_k = p.K / BK, n0 = walk.n_blk * BN;
     std::vector<float> d((size_t)64 * BN);               // the warpgroup's accumulator fragments
     std::vector<float> s1(BN, 0.f), s2(BN, 0.f);         // registers of the column owners t < BN
-    Ring st;
+    Ring st, rs;
     for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step) {
       int prev = 0;
       for (int kb = 0; kb < num_k; kb++) {
@@ -171,6 +196,7 @@ struct CTA {
       release(prev);                                       // wgmma.wait_group 0
       // (ct == 0: cp.async.bulk.wait_group.read 0 — the modelled store is synchronous)
       cons.sync();
+      if (p.res) res_full.wait(rs.ph);
       for (int w = 0; w < 4; w++)
         for (int lane = 0; lane < 32; lane++) {
           const int frag_row = wg * 64 + w * 16 + (lane >> 2);
@@ -178,17 +204,29 @@ struct CTA {
             const int col = 8 * j + 2 * (lane & 3);
             for (int i = 0; i < 2; i++) {
               const int row = frag_row + 8 * i;
-              const uint16_t pair[2] = {f2bf(d[(size_t)(row - wg * 64) * BN + col]), f2bf(d[(size_t)(row - wg * 64) * BN + col + 1])};
+              float* v = &d[(size_t)(row - wg * 64) * BN + col];
+              if (p.res) {
+                uint16_t r2[2];
+                memcpy(r2, sRes.data() + stage_elem_byte(col, row), 4);
+                const uint32_t bits = (uint32_t)sMask[mask_byte(BN, col, row)] >> (col & 7);
+                if (bits & 1u) v[0] += bf2f(r2[0]);
+                if (bits & 2u) v[1] += bf2f(r2[1]);
+              }
+              const uint16_t pair[2] = {f2bf(v[0]), f2bf(v[1])};
               memcpy(sOut.data() + stage_elem_byte(col, row), pair, 4);
             }
           }
         }
+      if (p.res) {
+        for (int w = 0; w < 4; w++) res_empty.arrive();   // lane 0 of each warp
+        rs.advance(1);
+      }
       cons.sync();
       if (wg == 0) {                                       // ct == 0 lives in warpgroup 0
         std::lock_guard<std::mutex> l(store_mu);
         for (int b = 0; b < BN / 64; b++) tma_store(sOut.data() + (size_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
       }
-      for (int t = 0; t < BN; t++)                         // col_owner
+      for (int t = 0; t < BN && !p.res; t++)               // col_owner
         for (int r = wg * 64; r < wg * 64 + 64; r++) {
           uint16_t h;
           memcpy(&h, sOut.data() + stage_elem_byte(t, r), 2);
@@ -197,10 +235,10 @@ struct CTA {
           s2[t] = std::fma(f, f, s2[t]);
         }
     }
-    if (wg == 1)
+    if (wg == 1 && !p.res)
       for (int t = 0; t < BN; t++) { sums[2 * t] = s1[t]; sums[2 * t + 1] = s2[t]; }
     cons.sync();
-    if (wg == 0 && walk.m_first < walk.num_m)
+    if (wg == 0 && !p.res && walk.m_first < walk.num_m)
       for (int t = 0; t < BN; t++) {
         p.partials[partial_index(walk.m_first, p.N, n0 + t)] = s1[t] + sums[2 * t];
         p.partials[partial_index(walk.m_first, p.N, n0 + t) + 1] = s2[t] + sums[2 * t + 1];
@@ -214,14 +252,19 @@ struct CTA {
   }
 };
 
-static int run_case(int M, int N, int K, int sms) {
+static int run_case(int M, int N, int K, int sms, bool res = false) {
   Problem p;
-  p.M = M; p.N = N; p.K = K; p.BN = N % 128 == 0 ? 128 : 64;
+  p.M = M; p.N = N; p.K = K; p.BN = N % 128 == 0 ? 128 : 64; p.res = res;
   p.X.resize((size_t)M * K); p.W.resize((size_t)N * K); p.Y.assign((size_t)M * N, 0xffff);
   uint32_t x = 12345u + (uint32_t)M * 7u + (uint32_t)N * 13u + (uint32_t)K;
   auto rnd = [&] { x = x * 1664525u + 1013904223u; return ((int)(x >> 20) % 2001 - 1000) / 1000.0f; };
   for (auto& v : p.X) v = f2bf(rnd());
   for (auto& v : p.W) v = f2bf(rnd() * 0.25f);
+  if (res) {
+    p.R.resize((size_t)M * N); p.mask.resize((size_t)M * N / 8);
+    for (auto& v : p.R) v = f2bf(rnd());
+    for (auto& v : p.mask) { x = x * 1664525u + 1013904223u; v = (uint8_t)(x >> 24); }
+  }
   // launch geometry exactly as launch<BN>() in gemm_bnstats.cu
   const int num_n = N / p.BN, num_m = (M + BM - 1) / BM;
   int groups = sms / num_n;
@@ -244,18 +287,20 @@ static int run_case(int M, int N, int K, int sms) {
     for (int n = 0; n < N; n++) {
       float acc = 0.f;
       for (int k = 0; k < K; k++) acc += bf2f(p.X[(size_t)m * K + k]) * bf2f(p.W[(size_t)n * K + k]);
+      if (res && ((p.mask[(size_t)m * (N / 8) + n / 8] >> (n % 8)) & 1)) acc += bf2f(p.R[(size_t)m * N + n]);
       const uint16_t want = f2bf(acc);
       const uint16_t got = p.Y[(size_t)m * N + n];
       if (std::fabs(bf2f(want) - bf2f(got)) > 1e-2f * std::fabs(bf2f(want)) + 1e-3f) bad++;   // summation order differs
       rs1[n] += bf2f(got);
       rs2[n] += (double)bf2f(got) * bf2f(got);
     }
-  for (int n = 0; n < N; n++) {
+  for (int n = 0; n < N && !res; n++) {
     double s1 = 0, s2 = 0;
     for (int g = 0; g < groups; g++) { s1 += p.partials[(size_t)g * 2 * N + 2 * n]; s2 += p.partials[(size_t)g * 2 * N + 2 * n + 1]; }
     if (std::fabs(s1 - rs1[n]) > 1e-3 * (std::fabs(rs1[n]) + 1.0) || std::fabs(s2 - rs2[n]) > 1e-3 * (rs2[n] + 1.0)) bad++;
   }
-  printf("M=%-5d N=%-4d K=%-4d BN=%-3d grid=%-3d groups=%-3d : %s\n", M, N, K, p.BN, grid, groups, bad ? "MISMATCH" : "ok");
+  printf("M=%-5d N=%-4d K=%-4d BN=%-3d grid=%-3d groups=%-3d %s: %s\n", M, N, K, p.BN, grid, groups, res ? "dgrad+res " : "",
+         bad ? "MISMATCH" : "ok");
   return bad;
 }
 
@@ -269,6 +314,10 @@ int main() {
   bad += run_case(2048, 256, 64, 4);       // 2 column blocks x 2 groups, 8 tiles per CTA, one k-block per tile
   bad += run_case(700, 192, 192, 6);       // BN = 64, 3 column blocks
   bad += run_case(384, 128, 576, 16);      // 9 k-blocks per tile, more SMs than tiles
+  // residual epilogue: one k-block per tile (the residual load races the next tile's operands), ragged M, ring wraps
+  bad += run_case(2048, 256, 64, 4, true);
+  bad += run_case(1000, 128, 320, 3, true);
+  bad += run_case(700, 256, 192, 2, true);
   bad += g_deadlocks.load();
   printf(bad ? "gemm_pipeline_model: FAILED (%d)\n" : "gemm_pipeline_model: all cases match the reference GEMM and column sums\n", bad);
   return bad ? 1 : 0;

@@ -12,7 +12,7 @@ from typing import List, Type
 import torch
 import torch.nn as nn
 
-from ..ops.fused_bn import bn_act, conv_bn_act
+from ..ops.fused_bn import ResidualLink, bn_act, conv_bn_act
 
 
 class BasicBlock(nn.Module):
@@ -50,9 +50,11 @@ class Bottleneck(nn.Module):
 
     def forward(self, x):
         idt = x if self.downsample is None else self.downsample(x)
-        out = conv_bn_act(self.conv1, self.bn1, x)      # 1x1: BN statistics can come from the GEMM epilogue (opt-in)
+        # residual == conv1's input: conv3's backward can hand the residual gradient to conv1's dgrad (ops/fused_bn.py)
+        link = ResidualLink() if self.downsample is None else None
+        out = conv_bn_act(self.conv1, self.bn1, x, link=link)   # 1x1: BN statistics can come from the GEMM epilogue
         out = bn_act(self.bn2, self.conv2(out))
-        return conv_bn_act(self.conv3, self.bn3, out, residual=idt)  # 1x1 + fused BN + add + ReLU
+        return conv_bn_act(self.conv3, self.bn3, out, residual=idt, link=link)  # 1x1 + fused BN + add + ReLU
 
 
 class _Downsample(nn.Sequential):

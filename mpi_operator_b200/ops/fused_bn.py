@@ -161,8 +161,39 @@ def bn_act(bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual: torch.Tensor = N
 # (csrc/kernels/gemm_bnstats.cu: TMA + wgmma). On by default (numerics: tests/test_zz_gemm_bnstats_gpu.py);
 # B200MPI_FUSED_CONV1X1=0 keeps cuDNN for the 1x1 convolutions.
 # Forward = 3 launches (GEMM+stats, finalize, apply) instead of conv + 3; backward = the fused BN backward kernels + two
-# library GEMMs (dgrad, wgrad).
+# library GEMMs (dgrad, wgrad), except for the residual hand-over below.
 _CONV1X1 = os.environ.get("B200MPI_FUSED_CONV1X1", "1") == "1"
+# In a residual block without downsample the block input x feeds both conv1 and the residual add, so autograd sums its two
+# gradients with an add kernel (read two tensors, write one) after bn3's backward has written mask3 ⊙ dv (dv = gradient of
+# the block output) as a tensor of its own. Through a ResidualLink, bn3's backward hands (dv, mask3) to conv1's node
+# instead, whose dgrad then runs on the wgmma kernel with mask3 ⊙ dv added in its epilogue: ~3 tensor passes less per block.
+# When x is itself the output of a fused conv+BN+ReLU (the previous block's bn3), the same epilogue also takes that BN's
+# backward reduction over the gradient it writes; the previous block's backward then skips its reduce pass (one tensor pass
+# less), provided the gradient it receives is that very tensor, unmodified.
+# B200MPI_FUSED_CONV1X1_BWD=0 keeps the autograd add and the reduce pass (A/B runs).
+_CONV1X1_BWD = os.environ.get("B200MPI_FUSED_CONV1X1_BWD", "1") == "1"
+
+
+class ResidualLink:
+    """Joins the conv3 node of a residual block (the one that adds the residual x) to the conv1 node that reads the same x.
+    conv1's fused forward arms it; conv3's backward fills ``dv`` / ``mask``; conv1's backward consumes them."""
+    __slots__ = ("armed", "dv", "mask")
+
+    def __init__(self):
+        self.armed, self.dv, self.mask = False, None, None
+
+
+class _HandedPartials:
+    """BN-backward partial rows taken by a later dgrad epilogue, and the identity of the gradient tensor they describe
+    (storage, version counter, shape, strides): the BN's backward may use them only for that exact tensor."""
+    __slots__ = ("partials", "parts", "key")
+
+    def __init__(self):
+        self.partials, self.parts, self.key = None, 0, None
+
+
+def _grad_key(t: torch.Tensor):
+    return (t.data_ptr(), t._version, tuple(t.shape), t.stride(), t.dtype)
 
 
 def _conv1x1_eligible(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor) -> bool:
@@ -179,7 +210,7 @@ def _conv1x1_eligible(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.
 
 class _Conv1x1BNAct(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, residual, w2d, weight, bias, running_mean, running_var, ws, eps, momentum, relu, direct):
+    def forward(ctx, x, residual, w2d, weight, bias, running_mean, running_var, ws, eps, momentum, relu, direct, link):
         from . import gemm_bnstats
         n, cin, h, w = x.shape
         cout = w2d.shape[0]
@@ -201,7 +232,13 @@ class _Conv1x1BNAct(torch.autograd.Function):
         _LAUNCHES += 3   # GEMM+stats, finalize, apply
         ctx.save_for_backward(x2d, w2d, yconv, mask, weight, save_mean, save_invstd, ws)
         ctx.relu, ctx.has_res, ctx.shape = relu, residual is not None, (n, cin, cout, h, w)
-        ctx.direct, ctx.wb = direct, (weight, bias)
+        ctx.direct, ctx.wb, ctx.link = direct, (weight, bias), link
+        # what the next fused 1x1 node needs to take this BN's backward reduction in its dgrad epilogue
+        ctx.handed = _HandedPartials() if residual is not None and relu and _CONV1X1_BWD else None
+        if ctx.handed is not None:
+            z._b200_bn_below = (yconv, mask, save_mean, ctx.handed)
+        below = getattr(x, "_b200_bn_below", None) if link is not None and residual is None else None
+        ctx.below = below if below is not None and below[0].shape == (m, cin) else None
         return z
 
     @staticmethod
@@ -209,38 +246,78 @@ class _Conv1x1BNAct(torch.autograd.Function):
         x2d, w2d, yconv, mask, weight, save_mean, save_invstd, ws = ctx.saved_tensors
         n, cin, cout, h, w = ctx.shape
         m = n * h * w
+        # this BN's reduction, if the next block's dgrad took it over exactly the gradient that arrives here
+        pre = None
+        if ctx.handed is not None and ctx.handed.partials is not None:
+            if ctx.handed.key == _grad_key(dz):
+                pre = (ctx.handed.partials, ctx.handed.parts)
+            ctx.handed.partials = None
         if dz.dtype != torch.bfloat16 or not dz.is_contiguous(memory_format=torch.channels_last):
             dz = dz.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
         dy = torch.empty(m, cout, dtype=torch.bfloat16, device=dz.device)          # gradient w.r.t. the convolution output
-        dres = torch.empty_like(dz, memory_format=torch.channels_last) if ctx.has_res else None
-        direct = (ctx.direct is not None and ctx.wb[0].grad is not None and ctx.wb[1].grad is not None
-                  and not getattr(ctx.direct, "accumulating", _never)())
+        accumulating = ctx.direct is not None and getattr(ctx.direct, "accumulating", _never)()
+        # residual side of a link: the residual gradient mask ⊙ dz goes to conv1's dgrad epilogue, not to autograd
+        hand_over = (ctx.link is not None and ctx.has_res and ctx.relu and ctx.needs_input_grad[1] and not accumulating
+                     and dz.data_ptr() % 16 == 0)
+        dres = torch.empty_like(dz, memory_format=torch.channels_last) if ctx.has_res and not hand_over else None
+        direct = (ctx.direct is not None and ctx.wb[0].grad is not None and ctx.wb[1].grad is not None and not accumulating)
         if direct:
             dw, db = ctx.wb[0].grad, ctx.wb[1].grad
         else:
             dw = torch.empty(cout, dtype=torch.float32, device=dz.device)
             db = torch.empty(cout, dtype=torch.float32, device=dz.device)
         stream = torch.cuda.current_stream(dz.device).cuda_stream
-        rc = _lib().b200mpi_bn_act_bwd(dz.data_ptr(), yconv.data_ptr(), _ptr(mask), dy.data_ptr(), _ptr(dres), weight.data_ptr(),
-                                       save_mean.data_ptr(), save_invstd.data_ptr(), dw.data_ptr(), db.data_ptr(), ws.data_ptr(),
-                                       m, cout, int(ctx.relu), stream)
-        if rc != 0:
-            raise RuntimeError(f"b200mpi_bn_act_bwd failed ({rc})")
         global _LAUNCHES
-        _LAUNCHES += 3
-        dx = (dy @ w2d).view(n, h, w, cin).permute(0, 3, 1, 2) if ctx.needs_input_grad[0] else None   # dgrad: [M,Cout] x [Cout,Cin]
-        dw2d = dy.t() @ x2d if ctx.needs_input_grad[2] else None                                          # wgrad: [Cout,M] x [M,Cin]
+        if pre is not None:
+            rc = _lib().b200mpi_bn_act_bwd_prestats(dz.data_ptr(), yconv.data_ptr(), _ptr(mask), dy.data_ptr(), _ptr(dres),
+                                                    weight.data_ptr(), save_mean.data_ptr(), save_invstd.data_ptr(), dw.data_ptr(),
+                                                    db.data_ptr(), ws.data_ptr(), pre[0].data_ptr(), pre[1], m, cout, int(ctx.relu),
+                                                    stream)
+            _LAUNCHES += 2
+        else:
+            rc = _lib().b200mpi_bn_act_bwd(dz.data_ptr(), yconv.data_ptr(), _ptr(mask), dy.data_ptr(), _ptr(dres), weight.data_ptr(),
+                                           save_mean.data_ptr(), save_invstd.data_ptr(), dw.data_ptr(), db.data_ptr(), ws.data_ptr(),
+                                           m, cout, int(ctx.relu), stream)
+            _LAUNCHES += 3
+        if rc != 0:
+            raise RuntimeError(f"b200mpi_bn_act_bwd{'_prestats' if pre is not None else ''} failed ({rc})")
+        if hand_over:
+            ctx.link.dv, ctx.link.mask = dz, mask
+        # input side of a link: the residual gradient of x, if the block's conv3 node handed it over
+        dv, mask_v = (ctx.link.dv, ctx.link.mask) if ctx.link is not None and not ctx.has_res else (None, None)
+        if dv is not None:
+            ctx.link.dv = ctx.link.mask = None
+        dx = None
+        if ctx.needs_input_grad[0] and dv is not None:
+            from . import gemm_bnstats
+            # W^T [Cin, Cout] is the K-major B operand of the kernel: a per-step copy of the (small) 1x1 weight
+            wt, dv2d = w2d.t().contiguous(), dv.permute(0, 2, 3, 1).reshape(m, cin)
+            if ctx.below is not None:
+                yb, mb, meanb, handed = ctx.below
+                dx, partials, parts = gemm_bnstats.dgrad_residual(dy, wt, dv2d, mask_v, below=(yb, mb, meanb))
+                dx = dx.view(n, h, w, cin).permute(0, 3, 1, 2)
+                handed.partials, handed.parts, handed.key = partials, parts, _grad_key(dx)
+            else:
+                dx = gemm_bnstats.dgrad_residual(dy, wt, dv2d, mask_v).view(n, h, w, cin).permute(0, 3, 1, 2)
+            _LAUNCHES += 1
+        elif ctx.needs_input_grad[0]:
+            dx = (dy @ w2d).view(n, h, w, cin).permute(0, 3, 1, 2)                    # dgrad: [M,Cout] x [Cout,Cin]
+        dw2d = dy.t() @ x2d if ctx.needs_input_grad[2] else None                      # wgrad: [Cout,M] x [M,Cin]
         if direct:
             ctx.direct(ctx.wb[0])
             ctx.direct(ctx.wb[1])
-            return dx, dres, dw2d, None, None, None, None, None, None, None, None, None
-        return dx, dres, dw2d, dw, db, None, None, None, None, None, None, None
+            return dx, dres, dw2d, None, None, None, None, None, None, None, None, None, None
+        return dx, dres, dw2d, dw, db, None, None, None, None, None, None, None, None
 
 
 def conv_bn_act(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual: torch.Tensor = None,
-                relu: bool = True) -> torch.Tensor:
+                relu: bool = True, link: ResidualLink = None) -> torch.Tensor:
     """``relu(bn(conv(x)) [+ residual])``. With B200MPI_FUSED_CONV1X1=1 an eligible 1x1 stride-1 convolution runs on the
-    wgmma GEMM whose epilogue already produces the BatchNorm statistics; everything else is ``bn_act(bn, conv(x), ...)``."""
+    wgmma GEMM whose epilogue already produces the BatchNorm statistics; everything else is ``bn_act(bn, conv(x), ...)``.
+
+    ``link``: one ResidualLink per residual block whose residual is the input of its first 1x1 convolution, passed to both
+    that call (``residual=None``: the link is armed if the fused dgrad can take the hand-over) and the call that adds the
+    residual (it hands the residual gradient over only to an armed link)."""
     if (_CONV1X1 and _conv1x1_eligible(conv, bn, x)
             and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape[0] == x.shape[0]
                                       and residual.shape[1] == conv.out_channels and residual.shape[2:] == x.shape[2:]))):
@@ -248,6 +325,12 @@ def conv_bn_act(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor
             residual = residual.contiguous(memory_format=torch.channels_last)
         _count_batch(bn)
         w2d = conv.weight.to(torch.bfloat16).reshape(conv.out_channels, conv.in_channels)
+        if link is not None and residual is None:
+            from . import gemm_bnstats
+            n, cin, h, w = x.shape
+            link.armed = _CONV1X1_BWD and gemm_bnstats.dgrad_res_supported(n * h * w, cin, conv.out_channels)
+        if link is not None and not link.armed:
+            link = None
         return _Conv1x1BNAct.apply(x, residual, w2d, bn.weight, bn.bias, bn.running_mean, bn.running_var, _ws(bn, x.device), bn.eps,
-                                   bn.momentum, relu, getattr(bn, "_b200_grad_ready", None))
+                                   bn.momentum, relu, getattr(bn, "_b200_grad_ready", None), link)
     return bn_act(bn, conv(x), residual=residual, relu=relu)

@@ -32,6 +32,9 @@ def lib() -> C.CDLL:
         L.b200mpi_gemm_bnstats_partial_floats.restype = C.c_size_t
         L.b200mpi_gemm_bnstats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_longlong,
                                            C.c_int, C.c_int, C.c_void_p]
+        L.b200mpi_gemm_dgrad_res_supported.argtypes = [C.c_longlong, C.c_int, C.c_int]
+        L.b200mpi_gemm_dgrad_res.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_longlong, C.c_int, C.c_int, C.c_void_p]
         _lib = L
     return _lib
 
@@ -51,13 +54,54 @@ def gemm_bnstats_raw(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tenso
     if not supported(m, n, k):
         raise ValueError(f"unsupported shape M={m} N={n} K={k} (N, K multiples of 64)")
     y = torch.empty(m, n, dtype=torch.bfloat16, device=x.device)
-    partials = torch.zeros(int(lib().b200mpi_gemm_bnstats_partial_floats(n)), dtype=torch.float32, device=x.device)
+    # the kernel writes every one of the `parts` rows it reports: no memset needed
+    partials = torch.empty(int(lib().b200mpi_gemm_bnstats_partial_floats(n)), dtype=torch.float32, device=x.device)
     parts = C.c_int(0)
     rc = lib().b200mpi_gemm_bnstats(x.data_ptr(), weight.data_ptr(), y.data_ptr(), partials.data_ptr(), C.byref(parts), m, n, k,
                                     torch.cuda.current_stream(x.device).cuda_stream)
     if rc != 0:
         raise RuntimeError(f"b200mpi_gemm_bnstats failed ({rc})")
     return y, partials[:parts.value * 2 * n].view(parts.value, n, 2), parts.value
+
+
+def dgrad_res_supported(m: int, n: int, k: int) -> bool:
+    return bool(lib().b200mpi_gemm_dgrad_res_supported(m, n, k))
+
+
+def dgrad_residual(dy: torch.Tensor, wt: torch.Tensor, r: torch.Tensor, mask: torch.Tensor, below=None):
+    """``dy [M,K] @ wt[N,K]^T + mask ⊙ r`` in one kernel (fp32 sum, one bf16 rounding): the input gradient of a 1x1
+    convolution plus the residual gradient of the same tensor. ``wt`` is the weight transposed to [Cin, Cout], ``r`` a
+    contiguous bf16 [M,N] tensor and ``mask`` its ReLU mask, one bit per element ([M, N/8] uint8, bit c%8 of byte c/8).
+
+    Without ``below`` returns dx [M,N]. With ``below = (xb, maskb, mean_b)`` — the saved input [M,N] bf16, ReLU mask and
+    saved mean [N] fp32 of the BatchNorm that produced the convolution's input — returns (dx, partials [parts, N, 2],
+    parts): that BN's backward reduction (sum g, sum g * (xb - mean_b), g = maskb ⊙ dx) for bn_act_bwd_prestats."""
+    if not (dy.is_cuda and dy.dtype == wt.dtype == r.dtype == torch.bfloat16 and mask.dtype == torch.uint8):
+        raise ValueError("dgrad_residual needs CUDA bf16 dy, wt, r and a uint8 mask")
+    m, k = dy.shape
+    n = wt.shape[0]
+    if (wt.shape[1] != k or r.shape != (m, n) or mask.numel() != m * n // 8 or not dy.is_contiguous() or not wt.is_contiguous()
+            or not r.is_contiguous() or not mask.is_contiguous()):
+        raise ValueError("expected contiguous dy [M,K], wt [N,K], r [M,N] and mask [M*N/8]")
+    if not dgrad_res_supported(m, n, k):
+        raise ValueError(f"unsupported shape M={m} N={n} K={k} (N multiple of 128, K of 64)")
+    dx = torch.empty(m, n, dtype=torch.bfloat16, device=dy.device)
+    xb = maskb = mean_b = partials = None
+    if below is not None:
+        xb, maskb, mean_b = below
+        if not (xb.dtype == torch.bfloat16 and xb.numel() == m * n and xb.is_contiguous() and maskb.dtype == torch.uint8
+                and maskb.numel() == m * n // 8 and maskb.is_contiguous() and mean_b.dtype == torch.float32 and mean_b.numel() == n):
+            raise ValueError("below = (xb [M,N] bf16, maskb [M*N/8] uint8, mean_b [N] fp32), contiguous")
+        partials = torch.empty(int(lib().b200mpi_gemm_bnstats_partial_floats(n)), dtype=torch.float32, device=dy.device)
+    parts = C.c_int(0)
+    p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    rc = lib().b200mpi_gemm_dgrad_res(dy.data_ptr(), wt.data_ptr(), dx.data_ptr(), r.data_ptr(), mask.data_ptr(), p(xb), p(maskb),
+                                      p(mean_b), p(partials), C.byref(parts), m, n, k, torch.cuda.current_stream(dy.device).cuda_stream)
+    if rc != 0:
+        raise RuntimeError(f"b200mpi_gemm_dgrad_res failed ({rc})")
+    if below is None:
+        return dx
+    return dx, partials[:parts.value * 2 * n].view(parts.value, n, 2), parts.value
 
 
 def conv1x1_with_stats(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
