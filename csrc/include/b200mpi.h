@@ -163,6 +163,19 @@ int b200mpi_allreduce_sgd_sym(b200mpi_comm_t comm, int grad_win, size_t grad_off
                               void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale,
                               float lr, float mu, float wd, int nesterov, int first_step,
                               b200mpi_algo_t algo, void* stream);
+/* Same step with parameter groups: vector i (4 fp32 elements) of the region is
+ * updated with {lr, mu, wd} = group_hyper[3*g .. 3*g+2], g = group_map[i].
+ * group_map is a device array of count/4 bytes for this region, every entry
+ * < num_groups; group_hyper a device table of num_groups x 3 floats, read at
+ * run time (a captured CUDA graph follows changes to it). Both NULL: exactly
+ * b200mpi_allreduce_sgd_sym. Groups need gdtype == B200MPI_F32 and
+ * 1 <= num_groups <= 256. Emulated mode: one map and table for all ranks. */
+int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t comm, int grad_win, size_t grad_off,
+                                     int param_win, size_t param_off, int lowp_win, size_t lowp_off,
+                                     void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale,
+                                     float lr, float mu, float wd, int nesterov, int first_step,
+                                     b200mpi_algo_t algo, void* stream,
+                                     const uint8_t* group_map, const float* group_hyper, int num_groups);
 size_t b200mpi_slice_elems(size_t count, int world, b200mpi_dtype_t dtype);
 /* Optional device-resident hyper-parameters {lr, momentum, weight_decay} (3 floats)
  * read by the fused kernels instead of the by-value arguments: a captured CUDA

@@ -615,12 +615,17 @@ k_allreduce_oneshot(const __grid_constant__ KArgs a0, const KArgs* __restrict__ 
 // its fp32 slice (momentum lives only on the owner: 1/world of the state) and
 // the all-gather half pushes the *updated parameters* to every rank. The
 // gradient never returns to HBM and the optimizer kernel disappears.
+// GROUPS (parameter groups, fp32 gradients only): vector i of the region takes
+// {lr, mu, wd} from row a.gmap[i] of the table a.ghyper instead of the
+// kernel-wide values. The flat layout pads every parameter to whole vectors,
+// so a vector never straddles two parameters and one byte per vector is exact.
 // ===========================================================================
-template <typename T, int MODE>
+template <typename T, int MODE, bool GROUPS = false>
 __global__ void __launch_bounds__(kThreads)
 k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu) {
   EMU_ARGS;
   constexpr int N = VecTraits<T>::N;
+  static_assert(!GROUPS || N == 4, "grouped SGD: one map entry per 4-element fp32 vector");
   const int rank = a.c.rank, world = a.c.world;
   uint32_t e = a.c.epoch[blockIdx.x];
   const size_t per = a.per, nvec = a.nvec;
@@ -642,6 +647,14 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
   constexpr int U = (MODE == MODE_NVLS) ? 4 : 2;
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x * U + threadIdx.x; i0 < lim; i0 += gstride() * U) {
     float gg[U][N];
+    int gid[U];  // GROUPS: group of each vector, loaded with the gradients so the table lookup below does not wait on it
+    if constexpr (GROUPS) {
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const size_t i = i0 + (size_t)u * blockDim.x;
+        gid[u] = i < lim ? __ldg(a.gmap + base + i) : 0;
+      }
+    }
     if (MODE == MODE_NVLS) {
       uint4 r[U];
 #pragma unroll
@@ -673,6 +686,11 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
       if (i >= lim) continue;
       float* g = gg[u];
       const size_t el = (base + i) * N;  // first element index of this vector
+      float vlr = lr, vmu = mu, vwd = wd;
+      if constexpr (GROUPS) {
+        const float* h = a.ghyper + 3 * gid[u];
+        vlr = __ldg(h); vmu = __ldg(h + 1); vwd = __ldg(h + 2);
+      }
       float p[N], m[N];
       const float* pl = reinterpret_cast<const float*>(a.param.p[rank]) + el;
       float* ml = a.mom + i * N;
@@ -687,10 +705,10 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
       }
   #pragma unroll
       for (int j = 0; j < N; j++) {
-        float gj = g[j] * a.scale + wd * p[j];
-        float mj = a.first_step ? gj : mu * m[j] + gj;
+        float gj = g[j] * a.scale + vwd * p[j];
+        float mj = a.first_step ? gj : vmu * m[j] + gj;
         m[j] = mj;
-        p[j] -= lr * (a.nesterov ? gj + mu * mj : mj);
+        p[j] -= vlr * (a.nesterov ? gj + vmu * mj : mj);
       }
   #pragma unroll
       for (int q = 0; q < N / 4; q++) {
@@ -1095,6 +1113,10 @@ cudaError_t launch_allreduce_oneshot(const Launch& l, const KArgs& a, int dtype)
 cudaError_t launch_allreduce_sgd(const Launch& l, const KArgs& a, int dtype, int mode) {
   if (mode == MODE_NVLS) DISPATCH_T(dtype, go(k_allreduce_sgd<T, MODE_NVLS>, l, a))
   DISPATCH_T(dtype, go(k_allreduce_sgd<T, MODE_P2P>, l, a))
+}
+cudaError_t launch_allreduce_sgd_groups(const Launch& l, const KArgs& a, int mode) {
+  if (mode == MODE_NVLS) return go(k_allreduce_sgd<float, MODE_NVLS, true>, l, a);
+  return go(k_allreduce_sgd<float, MODE_P2P, true>, l, a);
 }
 cudaError_t launch_allgather(const Launch& l, const KArgs& a) { return go(k_allgather, l, a); }
 cudaError_t launch_allgather_sym(const Launch& l, const KArgs& a, int mode) {

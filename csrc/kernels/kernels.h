@@ -11,8 +11,16 @@ namespace b200mpi {
 struct KArgs {
   DevComm c;
   Win buf;          // staging region or symmetric user region (per-rank bases)
-  const char* in;   // user input  (nullptr: data already in buf)
-  char* out;        // user output (nullptr: result stays in buf)
+  // The grouped fused SGD reads no user pointers, so its two tables share these slots: KArgs keeps its size, and with
+  // it the stride of the emulated ranks' argument array that every kernel indexes.
+  union {
+    const char* in;        // user input  (nullptr: data already in buf)
+    const uint8_t* gmap;   // grouped SGD: group id of each fp32 vector of the region, indexed like `buf`
+  };
+  union {
+    char* out;             // user output (nullptr: result stays in buf)
+    const float* ghyper;   // grouped SGD: device table [G][3] of {lr, mu, wd}
+  };
   size_t nbytes;    // payload bytes of one logical unit (op specific)
   size_t nvec;      // 16-byte vectors in the logical buffer
   size_t per;       // vectors per rank slice / slot
@@ -82,6 +90,8 @@ enum : int { PIPE_ALLREDUCE = 0, PIPE_ALLGATHER = 1, PIPE_REDUCE_SCATTER = 2, PI
 cudaError_t launch_pipe(const Launch& l, const KArgs& a, int kind, int dtype, int mode);
 cudaError_t launch_allreduce_oneshot(const Launch& l, const KArgs& a, int dtype);
 cudaError_t launch_allreduce_sgd(const Launch& l, const KArgs& a, int dtype, int mode);
+// per-vector hyper-parameters from a.gmap / a.ghyper; fp32 gradients only
+cudaError_t launch_allreduce_sgd_groups(const Launch& l, const KArgs& a, int mode);
 cudaError_t launch_allgather(const Launch& l, const KArgs& a);
 cudaError_t launch_allgather_sym(const Launch& l, const KArgs& a, int mode);
 cudaError_t launch_broadcast_sym(const Launch& l, const KArgs& a, int mode);

@@ -1128,6 +1128,18 @@ size_t b200mpi_slice_elems(size_t count, int world, b200mpi_dtype_t dtype) {
 int b200mpi_allreduce_sgd_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
                               void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, float lr, float mu,
                               float wd, int nesterov, int first_step, b200mpi_algo_t algo, void* stream) {
+  return b200mpi_allreduce_sgd_sym_groups(c, gwin, goff, pwin, poff, lwin, loff, momentum, count, gdtype, scale, lr, mu, wd,
+                                          nesterov, first_step, algo, stream, nullptr, nullptr, 0);
+}
+
+int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
+                                     void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, float lr, float mu,
+                                     float wd, int nesterov, int first_step, b200mpi_algo_t algo, void* stream,
+                                     const uint8_t* group_map, const float* group_hyper, int num_groups) {
+  const bool groups = group_map != nullptr;
+  if (groups != (group_hyper != nullptr)) return fail(B200MPI_ERR_INVALID, "allreduce_sgd: group map and group table must be given together");
+  if (groups && (num_groups < 1 || num_groups > 256)) return fail(B200MPI_ERR_INVALID, "allreduce_sgd: num_groups must be in [1, 256]");
+  if (groups && gdtype != B200MPI_F32) return fail(B200MPI_ERR_INVALID, "allreduce_sgd: parameter groups need fp32 gradients");
   if (count == 0) return 0;
   const size_t n = gdtype == B200MPI_F32 ? 4 : 8;
   auto okwin = [&](int w) { return w >= 0 && w < (int)c->wins.size() && c->wins[w].live; };
@@ -1153,9 +1165,13 @@ int b200mpi_allreduce_sgd_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin,
     a.nbytes = count * esize(gdtype); a.nvec = nvec; a.per = per;
     a.scale = scale; a.lr = lr; a.mu = mu; a.wd = wd; a.nesterov = nesterov; a.first_step = first_step;
     a.hyper = c->hyper;
+    a.gmap = group_map;      // emulated ranks share one read-only map and table
+    a.ghyper = group_hyper;
   }
   return run(c, (cudaStream_t)stream, blocks, "allreduce_sgd", count * esize(gdtype), mode == MODE_NVLS ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT, args,
-             [&](const Launch& l, const KArgs& a) { return launch_allreduce_sgd(l, a, gdtype, mode); });
+             [&](const Launch& l, const KArgs& a) {
+               return groups ? launch_allreduce_sgd_groups(l, a, mode) : launch_allreduce_sgd(l, a, gdtype, mode);
+             });
 }
 
 int b200mpi_set_hyper_ptr(b200mpi_comm_t c, const float* p) { c->hyper = p; return 0; }

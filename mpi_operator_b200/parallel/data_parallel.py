@@ -37,6 +37,42 @@ def _align(n: int, a: int) -> int:
     return (n + a - 1) // a * a
 
 
+MAX_PARAM_GROUPS = 256   # the fused kernel's group map holds one byte per vector
+_GROUP_KEYS = {"params", "lr", "momentum", "weight_decay", "nesterov"}
+
+
+def _resolve_param_groups(model: nn.Module, param_groups: Optional[list], lr: float, momentum: float, weight_decay: float,
+                          nesterov: bool):
+    """torch-style ``param_groups`` -> (members, values): group 0 holds the trainable parameters no group lists, with the
+    trainer-level values; group k >= 1 is ``param_groups[k - 1]``, its missing keys taken from the trainer."""
+    trainable = [p for p in model.parameters() if p.requires_grad]
+    groups = list(param_groups or [])
+    if len(groups) + 1 > MAX_PARAM_GROUPS:
+        raise ValueError(f"{len(groups)} parameter groups: at most {MAX_PARAM_GROUPS - 1} besides the implicit group 0")
+    known = {id(p) for p in trainable}
+    taken = set()
+    members, values = [], [[lr, momentum, weight_decay]]
+    for k, g in enumerate(groups):
+        if not isinstance(g, dict) or "params" not in g:
+            raise ValueError(f"parameter group {k}: expected a dict with a 'params' entry")
+        unknown = set(g) - _GROUP_KEYS
+        if unknown:
+            raise ValueError(f"parameter group {k}: unsupported keys {sorted(unknown)} (lr, momentum, weight_decay)")
+        if "nesterov" in g and bool(g["nesterov"]) != bool(nesterov):
+            raise ValueError(f"parameter group {k}: nesterov is a trainer-wide setting ({nesterov}), not per group")
+        ps = [g["params"]] if isinstance(g["params"], torch.Tensor) else list(g["params"])
+        for p in ps:
+            if id(p) not in known:
+                raise ValueError(f"parameter group {k}: a tensor of shape {tuple(p.shape)} is not a trainable parameter of the model")
+            if id(p) in taken:
+                raise ValueError(f"parameter group {k}: a parameter of shape {tuple(p.shape)} is listed twice")
+            taken.add(id(p))
+        members.append(ps)
+        values.append([float(g.get("lr", lr)), float(g.get("momentum", momentum)), float(g.get("weight_decay", weight_decay))])
+    members.insert(0, [p for p in trainable if id(p) not in taken])
+    return members, values
+
+
 @dataclass
 class Bucket:
     index: int
@@ -58,7 +94,10 @@ class FlatModelState:
     (``lowp_win``). Forward then needs no per-layer fp32->bf16 weight cast and backward no
     bf16->fp32 gradient cast + accumulate: ~3 small kernels per layer disappear from the step."""
 
-    def __init__(self, module: nn.Module, comm: Communicator, bucket_bytes: int = 32 << 20, bf16_params: bool = False):
+    def __init__(self, module: nn.Module, comm: Communicator, bucket_bytes: int = 32 << 20, bf16_params: bool = False,
+                 group_of: Optional[dict] = None):
+        """``group_of`` (parameter -> group index, missing: 0) builds ``group_map``: one uint8 group id per 4-element
+        vector of the flat buffers, which the grouped fused SGD kernel reads per vector."""
         self.comm = comm
         self.bf16_params = bf16_params
         params = [p for p in module.parameters() if p.requires_grad]
@@ -131,6 +170,19 @@ class FlatModelState:
                 p.grad = gv
         for b in self.buckets:
             b.momentum = torch.zeros(comm.slice_elems(b.numel, torch.float32), device=self.flat_param.device)
+        self.group_map: Optional[torch.Tensor] = None
+        if group_of is not None:
+            # every slot starts on a vector and is padded to whole vectors, so each vector lies in one parameter; its padding
+            # takes that parameter's group, the bucket tails (zeros in every buffer) group 0
+            gmap = torch.zeros(self.total // 4, dtype=torch.uint8)
+            for p in params:
+                start = self.param_slot[p][1]
+                gmap[start // 4:(start + _align(p.numel(), pad)) // 4] = group_of.get(p, 0)
+            self.group_map = gmap.to(self.flat_param.device)
+
+    def bucket_group_map(self, b: Bucket) -> torch.Tensor:
+        """The slice of ``group_map`` covering bucket ``b`` (``b.start`` and ``b.numel`` are multiples of 8 elements)."""
+        return self.group_map[b.start // 4:(b.start + b.numel) // 4]
 
     def broadcast_parameters(self, root: int = 0) -> None:
         """K3: rank-0 state to everyone (tensorflow_mnist.py:143)."""
@@ -180,13 +232,25 @@ class DataParallelTrainer:
     pinned host tensors), forward + backward under bf16 autocast, bucketed fused
     allreduce+SGD on the comm stream overlapped with backward, and leaves the
     loss on the device (``float(loss)`` is the D2H read).
+
+    ``param_groups`` takes ``torch.optim.SGD``-style groups, e.g. no weight decay on BatchNorm and biases::
+
+        no_wd = [p for n, p in model.named_parameters() if p.dim() == 1]
+        trainer = DataParallelTrainer(model, loss_fn, comm, lr=0.1, weight_decay=5e-5,
+                                      param_groups=[{"params": no_wd, "weight_decay": 0.0}])
+
+    Each group may set ``lr``, ``momentum`` and ``weight_decay``; missing keys take the trainer-level values. Trainable
+    parameters in no group form group 0 with the trainer-level values, so the groups given are 1, 2, ... in
+    ``trainer.param_groups`` and ``set_lr(lr, group=k)``. All three optimizer paths (fused kernel, ``fused_optimizer=False``,
+    ``comm_backend="nccl"``) apply the same per-group update.
     """
 
     def __init__(self, model: nn.Module, loss_fn: Callable, comm: Communicator, *, lr: float, momentum: float = 0.9,
                  weight_decay: float = 0.0, nesterov: bool = False, bucket_bytes: Optional[int] = None,
                  autocast_dtype: Optional[torch.dtype] = torch.bfloat16, channels_last: bool = True,
                  cuda_graph: bool = True, fused_optimizer: bool = True, algo: Optional[str] = None,
-                 comm_backend: str = "b200mpi", bf16_params: Optional[bool] = None, async_h2d: Optional[bool] = None):
+                 comm_backend: str = "b200mpi", bf16_params: Optional[bool] = None, async_h2d: Optional[bool] = None,
+                 param_groups: Optional[list] = None):
         self.comm = comm
         self.device = torch.device("cuda", comm.device) if comm.device != "cpu" else torch.device("cpu")
         self._cuda = self.device.type == "cuda"
@@ -209,12 +273,20 @@ class DataParallelTrainer:
             model = model.to(memory_format=torch.channels_last)
         self.model = model
         bucket_bytes = bucket_bytes or int(os.environ.get("B200MPI_BUCKET_BYTES", 32 << 20))
-        self.state = FlatModelState(model, comm, bucket_bytes, bf16_params=self.bf16_params)
+        names = {p: n for n, p in model.named_parameters()}
+        self._has_groups = param_groups is not None
+        members, values = _resolve_param_groups(model, param_groups, lr, momentum, weight_decay, nesterov)
+        self._group_names = [[names[p] for p in ps] for ps in members]
+        self._group_vals = values        # host copy of group_hyper, [[lr, momentum, weight_decay], ...]
+        group_of = {p: k for k, ps in enumerate(members) for p in ps} if self._has_groups else None
+        self.state = FlatModelState(model, comm, bucket_bytes, bf16_params=self.bf16_params, group_of=group_of)
         self.state.broadcast_parameters(0)
         # {lr, momentum, weight_decay} on the device: graph replays follow schedules
         self.hyper = torch.tensor([lr, momentum, weight_decay], device=self.device, dtype=torch.float32)
         comm.set_hyper(self.hyper)
         self._lr, self._mu, self._wd = lr, momentum, weight_decay
+        # with param_groups: one {lr, momentum, weight_decay} row per group on the device, read by the kernels the same way
+        self.group_hyper = torch.tensor(values, device=self.device, dtype=torch.float32) if self._has_groups else None
         self.comm_stream = torch.cuda.Stream(device=self.device, priority=-1) if self._cuda else None
         self._graph: Optional[torch.cuda.CUDAGraph] = None
         self._static_x = self._static_y = None
@@ -258,9 +330,28 @@ class DataParallelTrainer:
             comm.host_barrier()
 
     # ---------------------------------------------------------- hyper --
-    def set_lr(self, lr: float) -> None:
-        self._lr = lr
-        self.hyper[0] = lr
+    def set_lr(self, lr: float, group: Optional[int] = None) -> None:
+        """Learning rate of every group (``group=None``) or of group ``group`` (an index into ``param_groups``; group 0
+        holds the trainer-level values). Takes effect from the next step, CUDA-graph replays included."""
+        if group is not None and not 0 <= group < len(self._group_vals):
+            raise IndexError(f"group {group} out of range: the trainer has {len(self._group_vals)} parameter groups")
+        if group is None or group == 0:
+            self._lr = lr
+            self.hyper[0] = lr
+        for k in (range(len(self._group_vals)) if group is None else (group,)):
+            self._group_vals[k][0] = lr
+        if self.group_hyper is not None:
+            if group is None:
+                self.group_hyper[:, 0] = lr
+            else:
+                self.group_hyper[group, 0] = lr
+
+    @property
+    def param_groups(self) -> list:
+        """``[{"params": [parameter names], "lr": ..., "momentum": ..., "weight_decay": ...}, ...]``, group 0 (parameters
+        in no given group, trainer-level values) first. A copy: change values with ``set_lr``."""
+        return [{"params": list(n), "lr": v[0], "momentum": v[1], "weight_decay": v[2]}
+                for n, v in zip(self._group_names, self._group_vals)]
 
     @property
     def launches_per_step(self) -> int:
@@ -323,6 +414,13 @@ class DataParallelTrainer:
             g = st.flat_grad[b.start:b.start + b.numel]
             if self.comm.world > 1:
                 self._dist.all_reduce(g, op=self._dist.ReduceOp.AVG)
+        elif self.fused and self._has_groups:
+            self.comm.allreduce_sgd_window(st.grad_win, b.start * 4, st.param_win, b.start * 4, b.momentum,
+                                           b.numel, torch.float32, lr=self._lr, momentum_coef=self._mu,
+                                           weight_decay=self._wd, nesterov=self.nesterov,
+                                           lowp_win=st.lowp_win, lowp_off=b.start * 2, algo=self.algo,
+                                           stream=self.comm_stream, group_map=st.bucket_group_map(b),
+                                           group_hyper=self.group_hyper)
         elif self.fused:
             self.comm.allreduce_sgd_window(st.grad_win, b.start * 4, st.param_win, b.start * 4, b.momentum,
                                            b.numel, torch.float32, lr=self._lr, momentum_coef=self._mu,
@@ -338,6 +436,18 @@ class DataParallelTrainer:
         st = self.state
         if not hasattr(self, "_flat_mom"):
             self._flat_mom = torch.zeros_like(st.flat_param)
+        if self._has_groups:
+            # the fused kernel's per-vector update: each 4-element vector takes its group's row of the table
+            if not hasattr(self, "_group_index"):
+                self._group_index = st.group_map.long()
+            h = self.group_hyper[self._group_index]
+            lr, mu, wd = h[:, 0:1], h[:, 1:2], h[:, 2:3]
+            p, m = st.flat_param.view(-1, 4), self._flat_mom.view(-1, 4)
+            g = st.flat_grad.view(-1, 4) + wd * p
+            m.mul_(mu).add_(g)
+            p.sub_(lr * (g + mu * m if self.nesterov else m))
+            st.refresh_lowp()
+            return
         g = st.flat_grad
         if self._wd:
             g = g.add(st.flat_param, alpha=self._wd)
@@ -550,17 +660,29 @@ class DataParallelTrainer:
             start, n = st.param_slot[p][1], p.numel()
             masters[names[p]] = st.flat_param[start:start + n].as_strided(p.size(), p.stride()).detach().cpu().contiguous()
             momentum[names[p]] = mom_flat[start:start + n].as_strided(p.size(), p.stride()).detach().cpu().contiguous()
-        return {"format": "b200mpi.DataParallelTrainer/1", "model": masters, "momentum": momentum,
-                "buffers": {n: b.detach().cpu().clone() for n, b in self.model.named_buffers()},
-                "hyper": {"lr": float(self.hyper[0]), "momentum": float(self.hyper[1]), "weight_decay": float(self.hyper[2]),
-                          "nesterov": bool(self.nesterov)},
-                "world_size_at_save": int(self.comm.world)}
+        sd = {"format": "b200mpi.DataParallelTrainer/1", "model": masters, "momentum": momentum,
+              "buffers": {n: b.detach().cpu().clone() for n, b in self.model.named_buffers()},
+              "hyper": {"lr": float(self.hyper[0]), "momentum": float(self.hyper[1]), "weight_decay": float(self.hyper[2]),
+                        "nesterov": bool(self.nesterov)},
+              "world_size_at_save": int(self.comm.world)}
+        if self._has_groups:
+            sd["param_groups"] = self.param_groups
+        return sd
 
     def load_state_dict(self, sd: dict, load_hyper: bool = True) -> None:
         """Restore ``state_dict()`` output in a trainer built on the same model class (any world size, with or without the bf16
-        shadow / fused optimizer). Not collective: every rank loads the same dictionary and keeps its own momentum shard."""
+        shadow / fused optimizer). Not collective: every rank loads the same dictionary and keeps its own momentum shard.
+        With ``load_hyper``, per-group values are restored when the checkpoint's parameter groups have the same members (by
+        name) as this trainer's; a checkpoint with groups into a trainer without them, or the reverse, is a ``ValueError``."""
         if sd.get("format") != "b200mpi.DataParallelTrainer/1":
             raise ValueError("not a DataParallelTrainer checkpoint")
+        if load_hyper and ("param_groups" in sd) != self._has_groups:
+            raise ValueError("parameter groups: the checkpoint has them and this trainer does not, or the reverse "
+                             "(load_hyper=False skips the hyper-parameters)")
+        if load_hyper and self._has_groups:
+            theirs = [sorted(g["params"]) for g in sd["param_groups"]]
+            if theirs != [sorted(n) for n in self._group_names]:
+                raise ValueError("parameter groups of the checkpoint have other members than this trainer's")
         st = self.state
         names = {p: n for n, p in self.model.named_parameters()}
         missing = [n for n in names.values() if n not in sd["model"]]
@@ -595,6 +717,10 @@ class DataParallelTrainer:
             h = sd["hyper"]
             self._lr, self._mu, self._wd = h["lr"], h["momentum"], h["weight_decay"]
             self.hyper.copy_(torch.tensor([self._lr, self._mu, self._wd], dtype=torch.float32))
+            self._group_vals[0] = [self._lr, self._mu, self._wd]
+            if self._has_groups:
+                self._group_vals = [[g["lr"], g["momentum"], g["weight_decay"]] for g in sd["param_groups"]]
+                self.group_hyper.copy_(torch.tensor(self._group_vals, dtype=torch.float32))
         if self._cuda:
             torch.cuda.synchronize(self.device)
 

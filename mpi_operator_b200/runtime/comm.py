@@ -328,10 +328,36 @@ class Communicator:
     def allreduce_sgd_window(self, grad_win: Window, grad_off: int, param_win: Window, param_off: int, momentum,
                              count: int, grad_dtype, lr: float, momentum_coef: float = 0.0, weight_decay: float = 0.0,
                              nesterov: bool = False, first_step: bool = False, scale: Optional[float] = None,
-                             lowp_win: Optional[Window] = None, lowp_off: int = 0, algo=None, stream=None) -> None:
-        """Fused gradient-average + SGD step; see b200mpi_allreduce_sgd_sym."""
+                             lowp_win: Optional[Window] = None, lowp_off: int = 0, algo=None, stream=None,
+                             group_map=None, group_hyper=None) -> None:
+        """Fused gradient-average + SGD step; see b200mpi_allreduce_sgd_sym.
+
+        Parameter groups (fp32 gradients only): ``group_map`` is a CUDA uint8 tensor of ``count // 4`` entries, the group of
+        each 4-element vector of this region (already offset to it), and ``group_hyper`` a contiguous CUDA float32 ``[G, 3]``
+        tensor of ``{lr, momentum, weight_decay}`` rows, read by the kernel at run time, which then replaces ``lr``,
+        ``momentum_coef``, ``weight_decay`` and ``set_hyper``'s tensor. Every map entry must be ``< G``; the kernel does not
+        check it. On an emulated communicator one map and one table serve every rank."""
         pm, _ = self._ptrs(momentum)
         s = (1.0 / self.world) if scale is None else float(scale)
+        if group_map is not None or group_hyper is not None:
+            torch = _torch()
+            if group_map is None or group_hyper is None:
+                raise B200MPIError("allreduce_sgd_window: group_map and group_hyper go together")
+            if grad_dtype != torch.float32:
+                raise B200MPIError("allreduce_sgd_window: parameter groups need float32 gradients")
+            dev = torch.device("cuda", self.device)
+            if not (group_map.device == dev and group_map.dtype == torch.uint8 and group_map.is_contiguous()
+                    and group_map.numel() == count // 4):
+                raise B200MPIError(f"allreduce_sgd_window: group_map must be a contiguous uint8 tensor of {count // 4} entries on {dev}")
+            if not (group_hyper.device == dev and group_hyper.dtype == torch.float32 and group_hyper.is_contiguous()
+                    and group_hyper.dim() == 2 and group_hyper.shape[1] == 3 and 1 <= group_hyper.shape[0] <= 256):
+                raise B200MPIError(f"allreduce_sgd_window: group_hyper must be a contiguous float32 [G, 3] tensor on {dev}, 1 <= G <= 256")
+            check(_lib.lib().b200mpi_allreduce_sgd_sym_groups(
+                self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm,
+                count, dtype_code(grad_dtype), s, lr, momentum_coef, weight_decay, int(nesterov), int(first_step),
+                resolve_algo(algo), _stream_ptr(stream), group_map.data_ptr(), group_hyper.data_ptr(),
+                int(group_hyper.shape[0])), "allreduce_sgd_sym_groups")
+            return
         check(_lib.lib().b200mpi_allreduce_sgd_sym(
             self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm,
             count, dtype_code(grad_dtype), s, lr, momentum_coef, weight_decay, int(nesterov), int(first_step),
