@@ -221,7 +221,8 @@ int b200mpi_bn_act_fwd(const void* x, const void* residual, void* y, void* mask,
                        float* save_invstd, float* workspace, long long M, int C, float eps, float momentum,
                        int relu, void* stream);
 /* Same as b200mpi_bn_act_fwd but the per-channel statistics arrive as `parts` rows of {sum, sum of squares} (2*C floats
- * per row, unshifted) produced by the epilogue of b200mpi_gemm_bnstats: no statistics pass over x. */
+ * per row) produced by the epilogue of b200mpi_gemm_bnstats with x its output: row p holds the sums of x - x[128 p, c]
+ * over the 128-row tiles p, p + parts, ... of x. No statistics pass over x. */
 int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, void* mask, const float* weight, const float* bias,
                                 float* running_mean, float* running_var, float* save_mean, float* save_invstd, float* workspace,
                                 const float* partials, int parts, long long M, int C, float eps, float momentum, int relu,

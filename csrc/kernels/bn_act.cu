@@ -26,12 +26,14 @@
 #include <stdlib.h>
 
 #include "../include/b200mpi.h"
+#include "gemm_bnstats_logic.h"
 
 namespace b200mpi {
 namespace bn {
 
 constexpr int kThreadsBN = 256;
 constexpr int kUnroll = 4;
+constexpr int kBlockPasses = 16;   // statistics pass: loop passes (kUnroll rows each) summed apart before they are added
 
 __device__ __forceinline__ void unpack8(const uint4& v, float* f) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -88,23 +90,43 @@ __device__ __forceinline__ void block_reduce_to_partial(float (&s1)[8], float (&
 // slots x 8 outputs, each slot walking rows slot, slot+32, ... with 4 loads in flight -> ceil(parts/128) rounds of L2
 // latency (3 for the maximum of 296 rows; the 8-warps-x-32-outputs layout needed 10).
 // Returns (for threads 0..7) the total for output blockIdx.x*8 + threadIdx.x.
+//
+// WALK: the rows come from the 1x1-GEMM epilogue (gemm_bnstats.cu) and are forward statistics {sum, sum of squares} of
+// x = Y, row p shifted by its own K_p = x[shift_row(p), c] and covering walk_rows(p, parts, M) rows (gemm_bnstats_logic.h).
+// Each row is moved onto the shift K_0 = x[0, c] exactly before it is added, with d = K_p - K_0 and n_p its row count:
+//   S1 += s1_p + n_p d,   S2 += s2_p + d (2 s1_p + n_p d)
+// so the totals are sums of (x - K_0), as the statistics pass of this file produces them.
 constexpr int kMergeOut = 8;
-__device__ __forceinline__ float merge_partials(const float* __restrict__ partials, int parts, int nout, int* out_index) {
+template <bool WALK>
+__device__ __forceinline__ float merge_row(const float* p, int b, int nout, int parts, int o, const __nv_bfloat16* x, float k0, int M) {
+  const float v = __ldcg(p + (size_t)b * nout);
+  if (!WALK) return v;
+  const int c = o >> 1;
+  const float s1 = __ldcg(p + (size_t)b * nout - (o & 1));   // the row's sum for this channel (== v for o even)
+  const float d = __bfloat162float(x[(size_t)b200mpi::gemm::shift_row(b) * (size_t)(nout >> 1) + c]) - k0;
+  const float n = (float)b200mpi::gemm::walk_rows(b, parts, M);
+  return (o & 1) ? fmaf(d, fmaf(n, d, 2.f * s1), v) : fmaf(n, d, v);
+}
+template <bool WALK>
+__device__ __forceinline__ float merge_partials(const float* __restrict__ partials, int parts, int nout, const __nv_bfloat16* __restrict__ x,
+                                                long long M, int* out_index) {
   __shared__ float sm[8][kMergeOut + 1];
   const int oi = threadIdx.x & (kMergeOut - 1), slot = threadIdx.x >> 3;   // 32 slots
   const int o = blockIdx.x * kMergeOut + oi;
   float acc = 0.f;
   if (o < nout) {
     const float* p = partials + o;
+    const float k0 = WALK ? __bfloat162float(x[o >> 1]) : 0.f;
+    const int m = (int)M;   // WALK: the GEMM takes M < 2^31
     float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
     int b = slot;
     for (; b + 96 < parts; b += 128) {
-      a0 += __ldcg(p + (size_t)b * nout);
-      a1 += __ldcg(p + (size_t)(b + 32) * nout);
-      a2 += __ldcg(p + (size_t)(b + 64) * nout);
-      a3 += __ldcg(p + (size_t)(b + 96) * nout);
+      a0 += merge_row<WALK>(p, b, nout, parts, o, x, k0, m);
+      a1 += merge_row<WALK>(p, b + 32, nout, parts, o, x, k0, m);
+      a2 += merge_row<WALK>(p, b + 64, nout, parts, o, x, k0, m);
+      a3 += merge_row<WALK>(p, b + 96, nout, parts, o, x, k0, m);
     }
-    for (; b < parts; b += 32) a0 += __ldcg(p + (size_t)b * nout);
+    for (; b < parts; b += 32) a0 += merge_row<WALK>(p, b, nout, parts, o, x, k0, m);
     acc = (a0 + a1) + (a2 + a3);
   }
   // the 4 slots of a warp that share an output: lanes oi, oi+8, oi+16, oi+24
@@ -133,46 +155,62 @@ k_bn_fwd_stats(const uint4* __restrict__ x, float* __restrict__ partials, long l
   for (int j = 0; j < 8; j++) s1[j] = s2[j] = 0.f;
   const long long m0 = (long long)blockIdx.x * rows_per_cta;
   const long long m1 = m0 + rows_per_cta < M ? m0 + rows_per_cta : M;
-  for (long long m = m0 + r; m < m1; m += (long long)rpp * kUnroll) {
-    uint4 v[kUnroll];
+  // Rows are summed in blocks of kBlockPasses loop passes, each block's sums then added to the totals: a thread can own
+  // thousands of rows (one CTA over a layer: ~6,300 at M = 200704, C = 64), and one fp32 chain over them loses ~1e-4 of
+  // the variance.
+  const long long step = (long long)rpp * kUnroll;
+  for (long long mb = m0 + r; mb < m1; mb += step * kBlockPasses) {
+    const long long me = mb + step * kBlockPasses < m1 ? mb + step * kBlockPasses : m1;
+    float t1[8], t2[8];
 #pragma unroll
-    for (int u = 0; u < kUnroll; u++) {
-      const long long mm = m + (long long)u * rpp;
-      if (mm < m1) v[u] = ldg_stream(x + mm * tpr + cg);
-    }
+    for (int j = 0; j < 8; j++) t1[j] = t2[j] = 0.f;
+    for (long long m = mb; m < me; m += step) {
+      uint4 v[kUnroll];
 #pragma unroll
-    for (int u = 0; u < kUnroll; u++) {
-      const long long mm = m + (long long)u * rpp;
-      if (mm < m1) {
-        float f[8];
-        unpack8(v[u], f);
+      for (int u = 0; u < kUnroll; u++) {
+        const long long mm = m + (long long)u * rpp;
+        if (mm < m1) v[u] = ldg_stream(x + mm * tpr + cg);
+      }
 #pragma unroll
-        for (int j = 0; j < 8; j++) {
-          const float d = f[j] - K[j];
-          s1[j] += d;
-          s2[j] = fmaf(d, d, s2[j]);
+      for (int u = 0; u < kUnroll; u++) {
+        const long long mm = m + (long long)u * rpp;
+        if (mm < m1) {
+          float f[8];
+          unpack8(v[u], f);
+#pragma unroll
+          for (int j = 0; j < 8; j++) {
+            const float d = f[j] - K[j];
+            t1[j] += d;
+            t2[j] = fmaf(d, d, t2[j]);
+          }
         }
       }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+      s1[j] += t1[j];
+      s2[j] += t2[j];
     }
   }
   block_reduce_to_partial(s1, s2, partials + (size_t)blockIdx.x * 2 * C, C, tpr, r, cg, rpp);
 }
 
-// grid = ceil(2C/32): merges the partial rows, then the threads owning the (S1,S2) pair of a channel
-// produce mean / invstd / running stats / affine coefficients a, b for the apply pass.
+// grid = ceil(2C/8): merges the partial rows (sums of x - x[0, c]; WALK: see merge_partials), then the threads owning the
+// (S1,S2) pair of a channel produce mean / invstd / running stats / affine coefficients a, b for the apply pass.
+template <bool WALK>
 __global__ void __launch_bounds__(kThreadsBN)
-k_bn_fwd_finalize(const __nv_bfloat16* __restrict__ x_row0, const float* __restrict__ partials, int parts, float* __restrict__ coef,
+k_bn_fwd_finalize(const __nv_bfloat16* __restrict__ x, const float* __restrict__ partials, int parts, float* __restrict__ coef,
                   long long M, int C, const float* __restrict__ weight, const float* __restrict__ bias, float* running_mean,
                   float* running_var, float* save_mean, float* save_invstd, float eps, float momentum) {
   int o;
-  const float tot = merge_partials(partials, parts, 2 * C, &o);
+  const float tot = merge_partials<WALK>(partials, parts, 2 * C, x, M, &o);
   if ((threadIdx.x >> 5) != 0) return;
   const float other = __shfl_xor_sync(0xffffffffu, tot, 1);  // lanes 2j / 2j+1 hold S1 / S2 of one channel
   if (threadIdx.x >= kMergeOut || o >= 2 * C || (o & 1)) return;
   const int cgi = o >> 4, j = (o & 15) >> 1, c = cgi * 8 + j;
   const float S1 = tot, S2 = other;
   const float inv_m = 1.0f / (float)M;
-  const float k = x_row0 ? __bfloat162float(x_row0[c]) : 0.f;  // nullptr: partials are plain (unshifted) sums
+  const float k = __bfloat162float(x[c]);  // the shift of the merged sums
   const float d = S1 * inv_m;
   const float mean = k + d;
   float var = fmaf(-d, d, S2 * inv_m);
@@ -290,7 +328,7 @@ k_bn_bwd_finalize(const float* __restrict__ partials, int parts, float* __restri
                   const float* __restrict__ weight, const float* __restrict__ save_mean, const float* __restrict__ save_invstd,
                   float* dweight, float* dbias) {
   int o;
-  const float tot = merge_partials(partials, parts, 2 * C, &o);
+  const float tot = merge_partials<false>(partials, parts, 2 * C, nullptr, M, &o);
   if ((threadIdx.x >> 5) != 0) return;
   const float other = __shfl_xor_sync(0xffffffffu, tot, 1);
   if (threadIdx.x >= kMergeOut || o >= 2 * C || (o & 1)) return;
@@ -400,8 +438,8 @@ int b200mpi_bn_act_fwd(const void* x, const void* residual, void* y, void* mask,
   long long rows;
   plan(M, C, kMaxParts, 2LL * C, &grid, &rows, reduce_chunk());
   k_bn_fwd_stats<<<grid, kThreadsBN, 0, s>>>((const uint4*)x, partials, M, C, rows);
-  k_bn_fwd_finalize<<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>((const __nv_bfloat16*)x, partials, grid, coef, M, C, weight, bias,
-                                                            running_mean, running_var, save_mean, save_invstd, eps, momentum);
+  k_bn_fwd_finalize<false><<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>((const __nv_bfloat16*)x, partials, grid, coef, M, C, weight,
+                                                                   bias, running_mean, running_var, save_mean, save_invstd, eps, momentum);
   plan(M, C, 1184, (residual ? 6LL : 4LL) * C, &grid, &rows, elem_chunk());
   if (relu && residual) k_bn_fwd_apply<true, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, (const uint4*)residual, (uint4*)y, (uint8_t*)mask, coef, M, C, rows);
   else if (relu) k_bn_fwd_apply<true, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, nullptr, (uint4*)y, (uint8_t*)mask, coef, M, C, rows);
@@ -410,20 +448,22 @@ int b200mpi_bn_act_fwd(const void* x, const void* residual, void* y, void* mask,
   return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
 }
 
-// Forward with the statistics already reduced to `parts` rows of per-channel {sum, sum of squares} (unshifted) by the
-// producer of x — the epilogue of the wgmma 1x1-convolution GEMM (gemm_bnstats.cu): finalize + apply only, the
-// statistics pass over x is gone.
+// Forward with the statistics already reduced to `parts` rows of per-channel {sum, sum of squares} by the producer of x —
+// the epilogue of the wgmma 1x1-convolution GEMM (gemm_bnstats.cu), which shifts row p by x[128 p, c] and walks the
+// 128-row tiles p, p + parts, ... (gemm_bnstats_logic.h): finalize + apply only, the statistics pass over x is gone.
 int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, void* mask, const float* weight, const float* bias,
                                 float* running_mean, float* running_var, float* save_mean, float* save_invstd, float* workspace,
                                 const float* partials, int parts, long long M, int C, float eps, float momentum, int relu,
                                 void* stream_) {
-  if (!b200mpi_bn_supported(M, C) || parts < 1 || !partials) return B200MPI_ERR_UNSUPPORTED;
+  if (!b200mpi_bn_supported(M, C) || parts < 1 || !partials || M >= (1LL << 31) - b200mpi::gemm::BM ||
+      (long long)(parts - 1) * b200mpi::gemm::BM >= M)
+    return B200MPI_ERR_UNSUPPORTED;
   cudaStream_t s = (cudaStream_t)stream_;
   float* coef = workspace;
   int grid;
   long long rows;
-  k_bn_fwd_finalize<<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>(nullptr, partials, parts, coef, M, C, weight, bias, running_mean,
-                                                            running_var, save_mean, save_invstd, eps, momentum);
+  k_bn_fwd_finalize<true><<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>((const __nv_bfloat16*)x, partials, parts, coef, M, C, weight,
+                                                                  bias, running_mean, running_var, save_mean, save_invstd, eps, momentum);
   plan(M, C, 1184, (residual ? 6LL : 4LL) * C, &grid, &rows, elem_chunk());
   if (relu && residual) k_bn_fwd_apply<true, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, (const uint4*)residual, (uint4*)y, (uint8_t*)mask, coef, M, C, rows);
   else if (relu) k_bn_fwd_apply<true, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, nullptr, (uint4*)y, (uint8_t*)mask, coef, M, C, rows);

@@ -3,8 +3,9 @@
 //   Y[M,N] = X[M,K] . W[N,K]^T      bf16 in, fp32 accumulate in registers, bf16 out   (NHWC activations: M = N*H*W,
 //                                                                                       K = Cin, N = Cout, W is the conv
 //                                                                                       weight as stored)
-//   partials[p][2n+0] += sum_m Y[m,n],  partials[p][2n+1] += sum_m Y[m,n]^2      (one row per CTA m-group, the layout the
-//                                                                                  BN finalize kernel of bn_act.cu merges)
+//   partials[p][2n+0] = sum_m (Y[m,n] - K),  partials[p][2n+1] = sum_m (Y[m,n] - K)^2,  K = Y[128 p, n]
+//                                                        (one row per CTA m-group over the rows it walks, shifted by the first
+//                                                         row it stores; bn_act.cu's prestats finalize merges the rows)
 //
 // The same kernel with RES = true is the data gradient of a residual block's first 1x1 convolution (b200mpi_gemm_dgrad_res):
 //   dX[M,N] = dY[M,K] . Wt[N,K]^T + mask ⊙ R    (R = gradient of the block output, mask = its 1-bit ReLU mask; no statistics)
@@ -266,7 +267,7 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const int t = ct & 127;                      // thread `t` of each warpgroup owns column n0 + t for the statistics
   const bool col_owner = t < BN;
   const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  float s1 = 0.f, s2 = 0.f;
+  float s1 = 0.f, s2 = 0.f, shift = 0.f;
   const float mu = (GST && col_owner) ? mean_b[n0 + t] : 0.f;
   float d[BN / 2] = {};
   Ring st, rs;
@@ -336,15 +337,27 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
     if (!RES && col_owner) {
-      // column sums of the bf16-rounded tile (what the BN apply pass will read back). Rows past M are zero-filled by TMA.
+      // column sums of the bf16-rounded tile (what the BN apply pass will read back), shifted by K_p = row 0 of the CTA's
+      // first tile (shift_row in gemm_bnstats_logic.h). Rows past M are zero-filled by TMA and would each add -K_p: skipped.
+      if (m_blk == m_first) {
+        uint16_t h;
+        asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(sOut + stage_elem_byte(t, 0)));
+        shift = __uint_as_float((uint32_t)h << 16);
+      }
+      // The tile's 64 rows are summed on their own and then added: a CTA can walk ~200 tiles (M = 200704, N = 2048), and
+      // one fp32 chain over all of its ~12,500 rows loses ~1e-4 of the variance.
+      const int r_end = min(wg * 64 + 64, M - m_blk * BM);
+      float t1 = 0.f, t2 = 0.f;
 #pragma unroll 8
-      for (int r = wg * 64; r < wg * 64 + 64; r++) {
+      for (int r = wg * 64; r < r_end; r++) {
         uint16_t h;
         asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(sOut + stage_elem_byte(t, r)));
-        const float f = __uint_as_float((uint32_t)h << 16);
-        s1 += f;
-        s2 = fmaf(f, f, s2);
+        const float f = __uint_as_float((uint32_t)h << 16) - shift;
+        t1 += f;
+        t2 = fmaf(f, f, t2);
       }
+      s1 += t1;
+      s2 += t2;
     }
     if (GST) {
       if (col_owner) {
@@ -482,8 +495,15 @@ int b200mpi_gemm_bnstats_supported(long long M, int N, int K) {
           N / (N % 128 == 0 ? 128 : 64) <= b200mpi::gemm::kMaxParts) ? 1 : 0;
 }
 
-// rows of per-column {sum, sum of squares} the kernel may write: one per m-group, at most one per SM
+// rows of per-column {sum, sum of squares} (shifted: see shift_row in gemm_bnstats_logic.h) the kernel may write: one per
+// m-group, at most one per SM
 size_t b200mpi_gemm_bnstats_partial_floats(int N) { return (size_t)b200mpi::gemm::kMaxParts * 2 * (size_t)N; }
+
+// rows of Y that partial row p of `parts` covers (its shift is Y[128 p, c]): the tile-walk rule of the kernel
+long long b200mpi_gemm_bnstats_walk_rows(int p, int parts, long long M) {
+  if (p < 0 || parts < 1 || M < 1 || M >= (1LL << 31) - b200mpi::gemm::BM) return 0;
+  return b200mpi::gemm::walk_rows(p, parts, (int)M);
+}
 
 // Y = X . W^T (bf16, row-major, X [M,K], W [N,K], Y [M,N], all 16-byte aligned) and partials[parts][2N]; *parts = rows written.
 int b200mpi_gemm_bnstats(const void* X, const void* W, void* Y, float* partials, int* parts, long long M, int N, int K, void* stream) {

@@ -59,5 +59,17 @@ B200_HD uint32_t mask_byte(int BN, int col, int r) { return (uint32_t)r * (uint3
 // partials[m_first][2 * global_column + {0: sum, 1: sum of squares}]
 B200_HD size_t partial_index(int m_first, int N, int global_col) { return (size_t)m_first * 2 * (size_t)N + 2 * (size_t)global_col; }
 
+// The forward statistics of partial row p are shifted sums, sum (y - K_p) and sum (y - K_p)^2, against K_p = Y[shift_row(p), c]:
+// the first row of the CTA's first tile, a value of the column itself, so that the sums do not cancel when |mean| >> std.
+B200_HD long long shift_row(int p) { return (long long)p * BM; }
+// Rows of Y that partial row p covers when `groups` m-groups walk the row tiles (TileWalk: m_first = p, m_step = groups):
+// tiles p, p + groups, ... < num_m, the last tile of the matrix holding only M - (num_m - 1) * BM rows (M < 2^31 - BM).
+B200_HD int walk_rows(int p, int groups, int M) {
+  const int num_m = (M + BM - 1) / BM;
+  if (p >= num_m) return 0;
+  const int last = (num_m - 1 - p) % groups == 0 ? num_m * BM - M : 0;
+  return ((num_m - 1 - p) / groups + 1) * BM - last;
+}
+
 }  // namespace gemm
 }  // namespace b200mpi

@@ -8,10 +8,11 @@
 // staging layout, column ownership, the partial-row addressing — is the SAME code as in the kernel
 // (csrc/kernels/gemm_bnstats_logic.h); the role loops are transcribed statement by statement from the kernel.
 // A grid of such CTAs runs over a problem and the result is compared with a plain triple loop: Y, and the per-column
-// sum / sum of squares merged over the partial rows. A protocol error shows up as a deadlock (watchdog) or wrong data.
+// shifted sum / sum of squares merged over the partial rows. A protocol error shows up as a deadlock (watchdog) or wrong data.
 //
 // What this cannot tell: whether the PTX wrappers mean what the model assumes (descriptor bits are cross-checked with
 // CuTe in gmma_desc_test.cu). `make test_gemm_model`; run by tests/test_native_cpu.py.
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -181,7 +182,7 @@ struct CTA {
     const TileWalk walk(cta, grid, num_n, p.M);
     const int num_k = p.K / BK, n0 = walk.n_blk * BN;
     std::vector<float> d((size_t)64 * BN);               // the warpgroup's accumulator fragments
-    std::vector<float> s1(BN, 0.f), s2(BN, 0.f);         // registers of the column owners t < BN
+    std::vector<float> s1(BN, 0.f), s2(BN, 0.f), shift(BN, 0.f);   // registers of the column owners t < BN
     Ring st, rs;
     for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step) {
       int prev = 0;
@@ -226,14 +227,24 @@ struct CTA {
         std::lock_guard<std::mutex> l(store_mu);
         for (int b = 0; b < BN / 64; b++) tma_store(sOut.data() + (size_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
       }
-      for (int t = 0; t < BN && !p.res; t++)               // col_owner
-        for (int r = wg * 64; r < wg * 64 + 64; r++) {
+      const int r_end = std::min(wg * 64 + 64, p.M - m_blk * BM);
+      for (int t = 0; t < BN && !p.res; t++) {             // col_owner
+        if (m_blk == walk.m_first) {
+          uint16_t h;
+          memcpy(&h, sOut.data() + stage_elem_byte(t, 0), 2);
+          shift[t] = bf2f(h);
+        }
+        float t1 = 0.f, t2 = 0.f;
+        for (int r = wg * 64; r < r_end; r++) {
           uint16_t h;
           memcpy(&h, sOut.data() + stage_elem_byte(t, r), 2);
-          const float f = bf2f(h);
-          s1[t] += f;
-          s2[t] = std::fma(f, f, s2[t]);
+          const float f = bf2f(h) - shift[t];
+          t1 += f;
+          t2 = std::fma(f, f, t2);
         }
+        s1[t] += t1;
+        s2[t] += t2;
+      }
     }
     if (wg == 1 && !p.res)
       for (int t = 0; t < BN; t++) { sums[2 * t] = s1[t]; sums[2 * t + 1] = s2[t]; }
@@ -252,7 +263,7 @@ struct CTA {
   }
 };
 
-static int run_case(int M, int N, int K, int sms, bool res = false) {
+static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mean = false) {
   Problem p;
   p.M = M; p.N = N; p.K = K; p.BN = N % 128 == 0 ? 128 : 64; p.res = res;
   p.X.resize((size_t)M * K); p.W.resize((size_t)N * K); p.Y.assign((size_t)M * N, 0xffff);
@@ -260,6 +271,9 @@ static int run_case(int M, int N, int K, int sms, bool res = false) {
   auto rnd = [&] { x = x * 1664525u + 1013904223u; return ((int)(x >> 20) % 2001 - 1000) / 1000.0f; };
   for (auto& v : p.X) v = f2bf(rnd());
   for (auto& v : p.W) v = f2bf(rnd() * 0.25f);
+  if (big_mean)   // input column 0 = 1 and weight column 0 = 100 + n: every output column has |mean| / std of about 50
+    for (int m = 0; m < M; m++) p.X[(size_t)m * K] = f2bf(1.f);
+  for (int n = 0; n < N && big_mean; n++) p.W[(size_t)n * K] = f2bf(100.f + n);
   if (res) {
     p.R.resize((size_t)M * N); p.mask.resize((size_t)M * N / 8);
     for (auto& v : p.R) v = f2bf(rnd());
@@ -294,10 +308,22 @@ static int run_case(int M, int N, int K, int sms, bool res = false) {
       rs1[n] += bf2f(got);
       rs2[n] += (double)bf2f(got) * bf2f(got);
     }
+  // the rows are shifted by Y[shift_row(g), n]: merge them onto K_0 = Y[0, n] the way bn_act.cu's prestats finalize does and
+  // compare with sum (y - K_0), sum (y - K_0)^2. Every row of Y must be counted exactly once by walk_rows.
+  long long covered = 0;
+  for (int g = 0; g < groups; g++) covered += walk_rows(g, groups, M);
+  if (covered != M) bad++;
   for (int n = 0; n < N && !res; n++) {
+    const double k0 = bf2f(p.Y[n]);
+    const double want1 = rs1[n] - M * k0, want2 = rs2[n] - 2 * k0 * rs1[n] + M * k0 * k0;
     double s1 = 0, s2 = 0;
-    for (int g = 0; g < groups; g++) { s1 += p.partials[(size_t)g * 2 * N + 2 * n]; s2 += p.partials[(size_t)g * 2 * N + 2 * n + 1]; }
-    if (std::fabs(s1 - rs1[n]) > 1e-3 * (std::fabs(rs1[n]) + 1.0) || std::fabs(s2 - rs2[n]) > 1e-3 * (rs2[n] + 1.0)) bad++;
+    for (int g = 0; g < groups; g++) {
+      const double d = bf2f(p.Y[(size_t)shift_row(g) * N + n]) - k0, rows = walk_rows(g, groups, M);
+      const double a1 = p.partials[(size_t)g * 2 * N + 2 * n], a2 = p.partials[(size_t)g * 2 * N + 2 * n + 1];
+      s1 += a1 + rows * d;
+      s2 += a2 + d * (2 * a1 + rows * d);
+    }
+    if (std::fabs(s1 - want1) > 1e-3 * (std::fabs(want1) + 1.0) || std::fabs(s2 - want2) > 1e-3 * (want2 + 1.0)) bad++;
   }
   printf("M=%-5d N=%-4d K=%-4d BN=%-3d grid=%-3d groups=%-3d %s: %s\n", M, N, K, p.BN, grid, groups, res ? "dgrad+res " : "",
          bad ? "MISMATCH" : "ok");
@@ -314,6 +340,7 @@ int main() {
   bad += run_case(2048, 256, 64, 4);       // 2 column blocks x 2 groups, 8 tiles per CTA, one k-block per tile
   bad += run_case(700, 192, 192, 6);       // BN = 64, 3 column blocks
   bad += run_case(384, 128, 576, 16);      // 9 k-blocks per tile, more SMs than tiles
+  bad += run_case(1000, 64, 128, 5, false, true);   // large column means, ragged M: the shifted sums and their merge
   // residual epilogue: one k-block per tile (the residual load races the next tile's operands), ragged M, ring wraps
   bad += run_case(2048, 256, 64, 4, true);
   bad += run_case(1000, 128, 320, 3, true);

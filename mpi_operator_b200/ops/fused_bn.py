@@ -28,6 +28,9 @@ def fused_bn_available(x: torch.Tensor, bn: torch.nn.BatchNorm2d) -> bool:
             and bn.track_running_stats and bn.momentum is not None):
         return False
     n, c, h, w = x.shape
+    # one value per channel: training-mode batch norm is undefined, and nn.BatchNorm2d's error should reach the caller
+    if n * h * w < 2:
+        return False
     return bool(_lib().b200mpi_bn_supported(n * h * w, c)) and x.is_contiguous(memory_format=torch.channels_last)
 
 
@@ -216,7 +219,7 @@ class _Conv1x1BNAct(torch.autograd.Function):
         cout = w2d.shape[0]
         m = n * h * w
         x2d = x.permute(0, 2, 3, 1).reshape(m, cin)      # a view: channels-last memory is [M, Cin] row-major
-        yconv, partials, parts = gemm_bnstats.gemm_bnstats_raw(x2d, w2d)
+        yconv, partials, parts = gemm_bnstats.gemm_bnstats_shifted(x2d, w2d)
         z = torch.empty((n, cout, h, w), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
         mask = torch.empty(m * cout // 8, dtype=torch.uint8, device=x.device) if relu else None
         save_mean = torch.empty(cout, dtype=torch.float32, device=x.device)

@@ -1,11 +1,18 @@
 """Python front-end of the wgmma 1x1-convolution GEMM with fused BatchNorm statistics
 (csrc/kernels/gemm_bnstats.cu -> lib/libb200mpi_gemm.so).
 
-    y, s1, s2 = conv1x1_with_stats(x, weight)
+    y, partials, parts = gemm_bnstats_raw(x, weight)       # partial rows of plain sums
+    y, partials, parts = gemm_bnstats_shifted(x, weight)   # the kernel's own rows, as BatchNorm merges them
 
 ``x``: channels-last bf16 activations viewed as [M = N*H*W, Cin]; ``weight``: the convolution weight [Cout, Cin]
-(``conv.weight.view(Cout, Cin)``) in bf16. Returns the bf16 output [M, Cout] and the per-channel sum / sum of squares
-of that output (fp32), i.e. what BatchNorm's statistics pass would compute by re-reading ``y`` from HBM.
+(``conv.weight.view(Cout, Cin)``) in bf16. Both return the bf16 output [M, Cout] and ``parts`` rows of per-channel sums of
+that output (fp32), i.e. what BatchNorm's statistics pass would compute by re-reading ``y`` from HBM. Partial row p covers
+the 128-row tiles p, p + parts, ... of ``y``.
+
+The kernel shifts row p by a value of its own column, ``y[128 p]``: it holds ``sum (y - y[128 p])`` and
+``sum (y - y[128 p])^2``, which keep the variance when |mean| >> std. ``b200mpi_bn_act_fwd_prestats`` merges those rows
+(ops/fused_bn.py). ``gemm_bnstats_raw`` converts them to plain ``sum y`` and ``sum y^2`` in float64, for callers that
+want the sums themselves.
 
 The kernel is compiled for sm_90a (H100); ops/fused_bn.py calls it for eligible 1x1 convolutions. The reference ships no
 kernels (SURVEY.md §2.2)."""
@@ -30,6 +37,8 @@ def lib() -> C.CDLL:
         L.b200mpi_gemm_bnstats_supported.argtypes = [C.c_longlong, C.c_int, C.c_int]
         L.b200mpi_gemm_bnstats_partial_floats.argtypes = [C.c_int]
         L.b200mpi_gemm_bnstats_partial_floats.restype = C.c_size_t
+        L.b200mpi_gemm_bnstats_walk_rows.argtypes = [C.c_int, C.c_int, C.c_longlong]
+        L.b200mpi_gemm_bnstats_walk_rows.restype = C.c_longlong
         L.b200mpi_gemm_bnstats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_longlong,
                                            C.c_int, C.c_int, C.c_void_p]
         L.b200mpi_gemm_dgrad_res_supported.argtypes = [C.c_longlong, C.c_int, C.c_int]
@@ -43,8 +52,9 @@ def supported(m: int, n: int, k: int) -> bool:
     return bool(lib().b200mpi_gemm_bnstats_supported(m, n, k))
 
 
-def gemm_bnstats_raw(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, int]:
-    """Runs the kernel; returns (y [M,N] bf16, partials [parts, N, 2] fp32, parts)."""
+def gemm_bnstats_shifted(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, int]:
+    """Runs the kernel; returns (y [M,N] bf16, partials [parts, N, 2] fp32, parts). Row p holds {sum (y - y[128 p]),
+    sum (y - y[128 p])^2} over the rows of the tiles p, p + parts, ... (csrc/kernels/gemm_bnstats_logic.h)."""
     if x.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16 or not x.is_cuda:
         raise ValueError("gemm_bnstats needs CUDA bf16 tensors")
     if x.dim() != 2 or weight.dim() != 2 or x.shape[1] != weight.shape[1] or not x.is_contiguous() or not weight.is_contiguous():
@@ -62,6 +72,23 @@ def gemm_bnstats_raw(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tenso
     if rc != 0:
         raise RuntimeError(f"b200mpi_gemm_bnstats failed ({rc})")
     return y, partials[:parts.value * 2 * n].view(parts.value, n, 2), parts.value
+
+
+def walk_rows(m: int, parts: int) -> list:
+    """Rows of y that each partial row covers: the 128-row tiles p, p + parts, ..., the last tile holding the rest of M
+    (the kernel's own rule, walk_rows in csrc/kernels/gemm_bnstats_logic.h)."""
+    return [int(lib().b200mpi_gemm_bnstats_walk_rows(p, parts, m)) for p in range(parts)]
+
+
+def gemm_bnstats_raw(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, int]:
+    """Runs the kernel; returns (y [M,N] bf16, partials [parts, N, 2] fp32, parts) with row p = {sum y, sum y^2} over the
+    rows that partial row covers. The kernel's shifted rows are moved to plain sums in float64, then rounded to fp32."""
+    y, partials, parts = gemm_bnstats_shifted(x, weight)
+    k = y[0:(parts - 1) * 128 + 1:128].double()                                   # each row's shift y[128 p]
+    n = torch.tensor(walk_rows(x.shape[0], parts), dtype=torch.float64, device=y.device)[:, None]
+    a1, a2 = partials[..., 0].double(), partials[..., 1].double()
+    partials.copy_(torch.stack([a1 + n * k, a2 + k * (2 * a1 + n * k)], -1))
+    return y, partials, parts
 
 
 def dgrad_res_supported(m: int, n: int, k: int) -> bool:
@@ -102,9 +129,3 @@ def dgrad_residual(dy: torch.Tensor, wt: torch.Tensor, r: torch.Tensor, mask: to
     if below is None:
         return dx
     return dx, partials[:parts.value * 2 * n].view(parts.value, n, 2), parts.value
-
-
-def conv1x1_with_stats(x: torch.Tensor, weight: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-    y, partials, _ = gemm_bnstats_raw(x, weight)
-    tot = partials.sum(0)
-    return y, tot[:, 0].contiguous(), tot[:, 1].contiguous()
