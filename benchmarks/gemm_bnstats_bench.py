@@ -38,6 +38,13 @@ def dgrad_bytes_removed(m: int, n: int) -> int:
     return 5 * t - (2 * t + t // 16)
 
 
+def eval_bytes(m: int, k: int, n: int, fused: bool) -> int:
+    """HBM bytes of an eval-mode 1x1 conv + BN + residual + ReLU. Fused: X, W, R read, Y written once. Library GEMM + the eval
+    kernel: the GEMM writes Y, the eval kernel reads it back with R and writes the output: two more [M, N] passes."""
+    x, w, t = 2 * m * k, 2 * n * k, 2 * m * n
+    return x + w + 2 * t + (0 if fused else 2 * t)
+
+
 def timeit(fn, flush, iters):
     for _ in range(3):
         fn()
@@ -113,8 +120,35 @@ def main():
                            "ours_gbs": round(nbytes / t_ours / 1e6, 1), "step_bytes_removed": blocks * dgrad_bytes_removed(m, n)})
         print(json.dumps(dgrad_rows[-1]), flush=True)
     print(json.dumps({"dgrad_residual_bytes_removed_per_step": removed}), flush=True)
+    # eval epilogue: conv + BatchNorm (running statistics) + residual + ReLU in the GEMM, against cuBLAS + the one-pass eval kernel
+    from mpi_operator_b200.runtime import _lib
+    eval_rows = []
+    for m, k, n in SHAPES:
+        x = torch.randn(m, k, device=dev, dtype=torch.bfloat16)
+        w = torch.randn(n, k, device=dev, dtype=torch.bfloat16) * (k ** -0.5)
+        r = torch.randn(m, n, device=dev, dtype=torch.bfloat16)
+        bn = torch.nn.BatchNorm2d(n).to(dev).eval()
+        z = torch.empty(m, n, device=dev, dtype=torch.bfloat16)
+
+        def ours_eval():
+            return gemm_bnstats.gemm_bn_eval(x, w, bn, r, True)
+
+        def library_eval():
+            y = x @ w.t()
+            rc = _lib.lib().b200mpi_bn_act_eval(y.data_ptr(), r.data_ptr(), z.data_ptr(), bn.weight.data_ptr(), bn.bias.data_ptr(),
+                                                bn.running_mean.data_ptr(), bn.running_var.data_ptr(), m, n, bn.eps, 1,
+                                                torch.cuda.current_stream().cuda_stream)
+            assert rc == 0, rc
+            return z
+        t_ours, t_lib = timeit(ours_eval, flush, a.iters), timeit(library_eval, flush, a.iters)
+        b_ours, b_lib = eval_bytes(m, k, n, True), eval_bytes(m, k, n, False)
+        eval_rows.append({"M": m, "K": k, "N": n, "ours_us": round(1e3 * t_ours, 1), "cublas_plus_eval_kernel_us": round(1e3 * t_lib, 1),
+                          "speedup": round(t_lib / t_ours, 2), "ours_bytes": b_ours, "library_bytes": b_lib,
+                          "ours_gbs": round(b_ours / t_ours / 1e6, 1), "ours_frac_hbm": round(b_ours / t_ours / 1e6 / peaks["hbm_gbs"], 3)})
+        print(json.dumps(eval_rows[-1]), flush=True)
     out = {"peaks": {k_: peaks[k_] for k_ in ("hbm_gbs", "bf16_tflops")}, "l2": "256 MiB buffer rewritten between iterations",
-           "iters": a.iters, "rows": rows, "dgrad_rows": dgrad_rows, "dgrad_residual_bytes_removed_per_step": removed}
+           "iters": a.iters, "rows": rows, "dgrad_rows": dgrad_rows, "dgrad_residual_bytes_removed_per_step": removed,
+           "eval_rows": eval_rows, "card": torch.cuda.get_device_name(0)}
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:

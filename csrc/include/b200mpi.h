@@ -227,6 +227,12 @@ int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, vo
                                 float* running_mean, float* running_var, float* save_mean, float* save_invstd, float* workspace,
                                 const float* partials, int parts, long long M, int C, float eps, float momentum, int relu,
                                 void* stream);
+/* Eval-mode forward: z = relu?(a x + b [+ residual]) with a = weight * rsqrt(running_var + eps) and b = bias - running_mean * a
+ * (weight / bias NULL: 1 / 0), in fp32 with one bf16 rounding. Reads the running statistics and writes z only: no mask, no
+ * workspace, no statistics. Same C as b200mpi_bn_supported, any M >= 1; x, residual, y 16-byte aligned. */
+int b200mpi_bn_act_eval(const void* x, const void* residual, void* y, const float* weight, const float* bias,
+                        const float* running_mean, const float* running_var, long long M, int C, float eps, int relu,
+                        void* stream);
 int b200mpi_bn_act_bwd(const void* dz, const void* x, const void* mask, void* dx, void* dres,
                        const float* weight, const float* save_mean, const float* save_invstd,
                        float* dweight, float* dbias, float* workspace, long long M, int C, int relu,

@@ -277,6 +277,56 @@ k_bn_fwd_apply(const uint4* __restrict__ x, const uint4* __restrict__ res, uint4
   }
 }
 
+// ------------------------------------------------------------------- eval ----
+// Eval-mode BatchNorm (+ residual) (+ ReLU): z = relu?(a x + b (+ r)), a = weight * rsqrt(running_var + eps),
+// b = bias - running_mean * a, in fp32 with one bf16 rounding. Each thread derives a, b for its 8 channels from the running
+// statistics itself, so the layer is one launch that writes z only: no mask, no workspace, no statistics.
+template <bool RELU, bool RES>
+__global__ void __launch_bounds__(kThreadsBN)
+k_bn_eval_apply(const uint4* __restrict__ x, const uint4* __restrict__ res, uint4* __restrict__ y, const float* __restrict__ weight,
+                const float* __restrict__ bias, const float* __restrict__ running_mean, const float* __restrict__ running_var,
+                float eps, long long M, int C, long long rows_per_cta) {
+  const int tpr = C >> 3, rpp = kThreadsBN / tpr;
+  const int r = threadIdx.x / tpr, cg = threadIdx.x % tpr;
+  float a[8], b[8];
+#pragma unroll
+  for (int j = 0; j < 8; j++) {
+    const int c = cg * 8 + j;
+    a[j] = (weight ? weight[c] : 1.f) * rsqrtf(running_var[c] + eps);
+    b[j] = (bias ? bias[c] : 0.f) - running_mean[c] * a[j];
+  }
+  const long long m0 = (long long)blockIdx.x * rows_per_cta;
+  const long long m1 = m0 + rows_per_cta < M ? m0 + rows_per_cta : M;
+  for (long long m = m0 + r; m < m1; m += (long long)rpp * kUnroll) {
+    uint4 v[kUnroll], w[kUnroll];
+#pragma unroll
+    for (int u = 0; u < kUnroll; u++) {
+      const long long mm = m + (long long)u * rpp;
+      if (mm < m1) {
+        v[u] = ldg_stream(x + mm * tpr + cg);
+        if (RES) w[u] = ldg_stream(res + mm * tpr + cg);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kUnroll; u++) {
+      const long long mm = m + (long long)u * rpp;
+      if (mm < m1) {
+        float f[8], g[8];
+        unpack8(v[u], f);
+        if (RES) unpack8(w[u], g);
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          float z = fmaf(a[j], f[j], b[j]);
+          if (RES) z += g[j];
+          if (RELU) z = z > 0.f ? z : 0.f;
+          f[j] = z;
+        }
+        stg_stream(y + mm * tpr + cg, pack8(f));
+      }
+    }
+  }
+}
+
 // --------------------------------------------------------------- backward ----
 template <bool RELU>
 __global__ void __launch_bounds__(kThreadsBN)
@@ -469,6 +519,25 @@ int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, vo
   else if (relu) k_bn_fwd_apply<true, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, nullptr, (uint4*)y, (uint8_t*)mask, coef, M, C, rows);
   else if (residual) k_bn_fwd_apply<false, true><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, (const uint4*)residual, (uint4*)y, nullptr, coef, M, C, rows);
   else k_bn_fwd_apply<false, false><<<grid, kThreadsBN, 0, s>>>((const uint4*)x, nullptr, (uint4*)y, nullptr, coef, M, C, rows);
+  return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
+}
+
+// Eval mode: running statistics only, read and never written; one launch, no workspace (any stream, CUDA-graph safe).
+int b200mpi_bn_act_eval(const void* x, const void* residual, void* y, const float* weight, const float* bias, const float* running_mean,
+                        const float* running_var, long long M, int C, float eps, int relu, void* stream_) {
+  if (!b200mpi_bn_supported(M, C)) return B200MPI_ERR_UNSUPPORTED;
+  if (!x || !y || !running_mean || !running_var || ((uintptr_t)x | (uintptr_t)y | (uintptr_t)residual) & 15 || !(eps >= 0.f))
+    return B200MPI_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream_;
+  int grid;
+  long long rows;
+  plan(M, C, 1184, (residual ? 6LL : 4LL) * C, &grid, &rows, elem_chunk());
+  const uint4 *xv = (const uint4*)x, *rv = (const uint4*)residual;
+  uint4* yv = (uint4*)y;
+  if (relu && residual) k_bn_eval_apply<true, true><<<grid, kThreadsBN, 0, s>>>(xv, rv, yv, weight, bias, running_mean, running_var, eps, M, C, rows);
+  else if (relu) k_bn_eval_apply<true, false><<<grid, kThreadsBN, 0, s>>>(xv, nullptr, yv, weight, bias, running_mean, running_var, eps, M, C, rows);
+  else if (residual) k_bn_eval_apply<false, true><<<grid, kThreadsBN, 0, s>>>(xv, rv, yv, weight, bias, running_mean, running_var, eps, M, C, rows);
+  else k_bn_eval_apply<false, false><<<grid, kThreadsBN, 0, s>>>(xv, nullptr, yv, weight, bias, running_mean, running_var, eps, M, C, rows);
   return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
 }
 

@@ -11,6 +11,10 @@
 //   dX[M,N] = dY[M,K] . Wt[N,K]^T + mask ⊙ R    (R = gradient of the block output, mask = its 1-bit ReLU mask; no statistics)
 // so that the residual gradient never exists as a tensor of its own and autograd adds nothing.
 //
+// With EVAL = true it is an eval-mode 1x1 convolution + BatchNorm (+ residual) (+ ReLU) (b200mpi_gemm_bn_eval):
+//   Y[M,N] = relu?(a[n] * (X . W^T)[m,n] + b[n] (+ R[m,n])),  a = gamma * rsqrt(running_var + eps),  b = beta - running_mean * a
+// summed in fp32 and rounded to bf16 once; no statistics (RES = R is present, loaded without a mask).
+//
 // Why: two thirds of ResNet's BatchNorm layers follow a 1x1 convolution. Their statistics pass re-reads the whole
 // convolution output from HBM; here the tile is still in shared memory when its column sums are taken, so the pass
 // disappears. The reference has no kernels at all (SURVEY.md §2.2) — this is part of the data plane the new framework adds.
@@ -159,7 +163,8 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 // in the layout k_bn_bwd_finalize merges (instead of the forward's sum / sum of squares).
 // The epilogue operands are TMA-loaded by the producer into a region of their own while the tile's last k-blocks run; with
 // GST the operand ring has 3 stages so that everything fits in shared memory.
-template <int BN, bool RES, bool GST>
+// EVAL (RES = a residual R without mask): a, b of the CTA's columns live in the kSums region.
+template <int BN, bool RES, bool GST, bool EVAL = false>
 struct Smem {
   static constexpr int kS = GST ? 3 : kStages;
   static constexpr uint32_t kBBytes = BN * BK * 2;
@@ -167,7 +172,7 @@ struct Smem {
   static constexpr uint32_t kOutBoxes = BN / 64;                  // TMA store boxes of [128 rows x 64 cols] (128 B inner)
   static constexpr uint32_t kOutBytes = kOutBoxes * kBoxBytes;
   static constexpr uint32_t kResBytes = RES ? kOutBytes : 0;      // residual tile, same swizzled layout as the staging
-  static constexpr uint32_t kMaskBytes = RES ? BM * BN / 8 : 0;
+  static constexpr uint32_t kMaskBytes = RES && !EVAL ? BM * BN / 8 : 0;
   static constexpr uint32_t kXbBytes = GST ? kOutBytes : 0;       // the lower BN's input tile, same layout
   static constexpr uint32_t kMaskBBytes = GST ? BM * BN / 8 : 0;
   static constexpr uint32_t kA = 0;
@@ -183,13 +188,14 @@ struct Smem {
   static constexpr uint32_t kDynamic = kTotal + 1024;             // slack to align the base to 1024 B (swizzle atoms)
 };
 
-template <int BN, bool RES, bool GST>
+template <int BN, bool RES, bool GST, bool EVAL = false>
 __global__ void __launch_bounds__(kThreads, 1)
 k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmY,
                const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmMask,
                const __grid_constant__ CUtensorMap tmXb, const __grid_constant__ CUtensorMap tmMaskB, const float* __restrict__ mean_b,
-               float* __restrict__ partials, int M, int N, int K, int num_n) {
-  using L = Smem<BN, RES, GST>;
+               float* __restrict__ partials, int M, int N, int K, int num_n, const float* __restrict__ bn_w,
+               const float* __restrict__ bn_b, const float* __restrict__ bn_rm, const float* __restrict__ bn_rv, float eps, int relu) {
+  using L = Smem<BN, RES, GST, EVAL>;
   constexpr int S = L::kS;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -217,7 +223,7 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
     }
     if (RES) {
       tma_prefetch_desc(&tmR);
-      tma_prefetch_desc(&tmMask);
+      if (!EVAL) tma_prefetch_desc(&tmMask);
       mbar_init(res_full, 1);
       mbar_init(res_empty, kConsumers / 32);       // one arrive per consumer warp once it has read the epilogue operands
     }
@@ -248,7 +254,7 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
           mbar_arrive_expect_tx(res_full, L::kResBytes + L::kMaskBytes + L::kXbBytes + L::kMaskBBytes);
 #pragma unroll
           for (int b = 0; b < (int)L::kOutBoxes; b++) tma_load_2d(sRes + (uint32_t)b * kBoxBytes, &tmR, res_full, n0 + b * 64, m_blk * BM);
-          tma_load_2d(sMask, &tmMask, res_full, n0 / 8, m_blk * BM);
+          if (!EVAL) tma_load_2d(sMask, &tmMask, res_full, n0 / 8, m_blk * BM);
           if (GST) {
 #pragma unroll
             for (int b = 0; b < (int)L::kOutBoxes; b++) tma_load_2d(sXb + (uint32_t)b * kBoxBytes, &tmXb, res_full, n0 + b * 64, m_blk * BM);
@@ -269,6 +275,13 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const int frag_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   float s1 = 0.f, s2 = 0.f, shift = 0.f;
   const float mu = (GST && col_owner) ? mean_b[n0 + t] : 0.f;
+  if (EVAL && wg == 0 && col_owner) {
+    // this CTA's columns for the whole kernel; read by the epilogue after its first consumer barrier
+    const int c = n0 + t;
+    const float a = (bn_w ? bn_w[c] : 1.f) * rsqrtf(bn_rv[c] + eps);
+    sums[t] = a;
+    sums[BN + t] = (bn_b ? bn_b[c] : 0.f) - bn_rm[c] * a;
+  }
   float d[BN / 2] = {};
   Ring st, rs;
   for (int m_blk = m_first; m_blk < num_m; m_blk += m_step) {
@@ -296,7 +309,37 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
 
     if (ct == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // previous tile's store has read the staging
     cons_bar_sync();                                                               // ... and its column sums are taken
-    if (RES) {
+    if (EVAL) {
+      // out = relu?(a * acc + b (+ R)) in fp32, rounded to bf16 once
+      if (RES) mbar_wait(res_full, rs.ph);
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) {
+        const int col = 8 * j + 2 * (lane & 3);
+        const float2 a = *reinterpret_cast<const float2*>(sums + col);
+        const float2 b = *reinterpret_cast<const float2*>(sums + BN + col);
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+          float v0 = fmaf(a.x, d[4 * j + 2 * i], b.x), v1 = fmaf(a.y, d[4 * j + 2 * i + 1], b.y);
+          if (RES) {
+            uint32_t r2;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r2) : "r"(sRes + stage_elem_byte(col, frag_row + 8 * i)) : "memory");
+            v0 += __uint_as_float(r2 << 16);
+            v1 += __uint_as_float(r2 & 0xffff0000u);
+          }
+          if (relu) {
+            v0 = v0 > 0.f ? v0 : 0.f;
+            v1 = v1 > 0.f ? v1 : 0.f;
+          }
+          d[4 * j + 2 * i] = v0;
+          d[4 * j + 2 * i + 1] = v1;
+        }
+      }
+      if (RES) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(res_empty);
+        rs.advance(1);
+      }
+    } else if (RES) {
       // out = acc + mask ⊙ R in fp32, rounded to bf16 once
       mbar_wait(res_full, rs.ph);
 #pragma unroll
@@ -336,7 +379,7 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       for (int b = 0; b < (int)L::kOutBoxes; b++) tma_store_2d(&tmY, sOut + (uint32_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
-    if (!RES && col_owner) {
+    if (!RES && !EVAL && col_owner) {
       // column sums of the bf16-rounded tile (what the BN apply pass will read back), shifted by K_p = row 0 of the CTA's
       // first tile (shift_row in gemm_bnstats_logic.h). Rows past M are zero-filled by TMA and would each add -K_p: skipped.
       if (m_blk == m_first) {
@@ -380,12 +423,12 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
       rs.advance(1);
     }
   }
-  if ((!RES || GST) && wg == 1 && col_owner) {
+  if ((!RES || GST) && !EVAL && wg == 1 && col_owner) {
     sums[2 * t] = s1;
     sums[2 * t + 1] = s2;
   }
   cons_bar_sync();
-  if ((!RES || GST) && wg == 0 && col_owner && m_first < num_m) {
+  if ((!RES || GST) && !EVAL && wg == 0 && col_owner && m_first < num_m) {
     float* row_out = partials + partial_index(m_first, N, n0 + t);
     row_out[0] = s1 + sums[2 * t];
     row_out[1] = s2 + sums[2 * t + 1];
@@ -445,14 +488,23 @@ static bool make_mask_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint
 
 // RES: R and mask are the residual operand of the dgrad epilogue; GST: Xb, maskB, mean_b are the lower BN's saved input,
 // ReLU mask and mean, and partials receive its backward partials; otherwise partials receive the column statistics.
-template <int BN, bool RES, bool GST>
+// EVAL: bn = {weight, bias, running_mean, running_var} of the eval-mode BatchNorm, R (RES) its residual, no mask, no partials.
+struct EvalBN {
+  const float *w, *b, *rm, *rv;
+  float eps;
+  int relu;
+};
+template <int BN, bool RES, bool GST, bool EVAL = false>
 static int launch(const void* X, const void* W, void* Y, float* partials, int* parts_out, const void* R, const void* mask, const void* Xb,
-                  const void* maskB, const float* mean_b, long long M, int N, int K, cudaStream_t s) {
+                  const void* maskB, const float* mean_b, long long M, int N, int K, cudaStream_t s, const EvalBN& bn = EvalBN{}) {
   CUtensorMap tmX, tmW, tmY, tmR, tmMask, tmXb, tmMaskB;
   if (!make_map(&tmX, X, (uint64_t)M, (uint64_t)K, BM) || !make_map(&tmW, W, (uint64_t)N, (uint64_t)K, BN) ||
       !make_map(&tmY, Y, (uint64_t)M, (uint64_t)N, BM))
     return B200MPI_ERR_CUDA;
-  if (RES) {
+  if (RES && EVAL) {
+    if (!make_map(&tmR, R, (uint64_t)M, (uint64_t)N, BM)) return B200MPI_ERR_CUDA;
+    tmMask = tmY;   // unused
+  } else if (RES) {
     if (!make_map(&tmR, R, (uint64_t)M, (uint64_t)N, BM) || !make_mask_map(&tmMask, mask, (uint64_t)M, (uint64_t)N / 8, BM, BN / 8))
       return B200MPI_ERR_CUDA;
   } else {
@@ -472,13 +524,13 @@ static int launch(const void* X, const void* W, void* Y, float* partials, int* p
   if (groups > num_m) groups = num_m;
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(k_gemm_bnstats<BN, RES, GST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)Smem<BN, RES, GST>::kDynamic) != cudaSuccess)
+    if (cudaFuncSetAttribute(k_gemm_bnstats<BN, RES, GST, EVAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)Smem<BN, RES, GST, EVAL>::kDynamic) != cudaSuccess)
       return B200MPI_ERR_CUDA;
     attr_set = true;
   }
-  k_gemm_bnstats<BN, RES, GST><<<groups * num_n, kThreads, Smem<BN, RES, GST>::kDynamic, s>>>(tmX, tmW, tmY, tmR, tmMask, tmXb, tmMaskB,
-                                                                                              mean_b, partials, (int)M, N, K, num_n);
+  k_gemm_bnstats<BN, RES, GST, EVAL><<<groups * num_n, kThreads, Smem<BN, RES, GST, EVAL>::kDynamic, s>>>(
+      tmX, tmW, tmY, tmR, tmMask, tmXb, tmMaskB, mean_b, partials, (int)M, N, K, num_n, bn.w, bn.b, bn.rm, bn.rv, bn.eps, bn.relu);
   if (parts_out) *parts_out = groups;
   return cudaGetLastError() == cudaSuccess ? 0 : B200MPI_ERR_CUDA;
 }
@@ -534,6 +586,28 @@ int b200mpi_gemm_dgrad_res(const void* dY, const void* Wt, void* dX, const void*
   if (!Xb) return launch<128, true, false>(dY, Wt, dX, nullptr, parts, R, mask, nullptr, nullptr, nullptr, M, N, K, (cudaStream_t)stream);
   if (!maskB || !mean_b || !partials) return B200MPI_ERR_INVALID;
   return launch<128, true, true>(dY, Wt, dX, partials, parts, R, mask, Xb, maskB, mean_b, M, N, K, (cudaStream_t)stream);
+}
+
+// Eval-mode 1x1 convolution + BatchNorm (+ residual) (+ ReLU): Y[M,N] = relu?(a * (X . W^T) + b (+ R)) with, per column,
+// a = weight * rsqrt(running_var + eps) and b = bias - running_mean * a (weight / bias nullptr: 1 / 0), summed in fp32 and
+// rounded to bf16 once. X [M,K], W [N,K], Y and R (nullptr: no residual) [M,N] bf16 row-major, 16-byte aligned. Reads the
+// running statistics only: no partial rows, no mask. Rows of Y past M are not written.
+int b200mpi_gemm_bn_eval_supported(long long M, int N, int K) { return b200mpi_gemm_bnstats_supported(M, N, K); }
+
+int b200mpi_gemm_bn_eval(const void* X, const void* W, void* Y, const void* R, const float* weight, const float* bias,
+                         const float* running_mean, const float* running_var, float eps, int relu, long long M, int N, int K,
+                         void* stream) {
+  using namespace b200mpi::gemm;
+  if (!b200mpi_gemm_bn_eval_supported(M, N, K)) return B200MPI_ERR_UNSUPPORTED;
+  if (((uintptr_t)X | (uintptr_t)W | (uintptr_t)Y | (uintptr_t)R) & 15) return B200MPI_ERR_INVALID;
+  if (!X || !W || !Y || !running_mean || !running_var || !(eps >= 0.f)) return B200MPI_ERR_INVALID;
+  const EvalBN bn{weight, bias, running_mean, running_var, eps, relu ? 1 : 0};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (N % 128 == 0)
+    return R ? launch<128, true, false, true>(X, W, Y, nullptr, nullptr, R, nullptr, nullptr, nullptr, nullptr, M, N, K, s, bn)
+             : launch<128, false, false, true>(X, W, Y, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, M, N, K, s, bn);
+  return R ? launch<64, true, false, true>(X, W, Y, nullptr, nullptr, R, nullptr, nullptr, nullptr, nullptr, M, N, K, s, bn)
+           : launch<64, false, false, true>(X, W, Y, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, M, N, K, s, bn);
 }
 
 }  // extern "C"

@@ -85,6 +85,9 @@ struct Problem {
   bool res = false;                // dgrad epilogue: Y = X.W^T + mask ⊙ R, no statistics
   std::vector<uint16_t> R;         // [M,N] bf16
   std::vector<uint8_t> mask;       // [M, N/8]: bit c%8 of byte c/8
+  bool eval = false;               // eval epilogue: Y = relu?(a . (X.W^T) + b (+ R)), R without mask, no statistics
+  bool relu = false;
+  std::vector<float> a, b;         // [N]: the eval-mode BatchNorm's per-column scale and shift
 };
 
 // ------------------------------------------------------------------- CTA ----
@@ -144,16 +147,18 @@ struct CTA {
         d[(size_t)m * BN + n] = acc;
       }
   }
-  // the residual tile ([128 x 64] SWIZZLE_128B boxes, zero fill past M) and its mask tile ([128 x BN/8] bytes, unswizzled)
+  // the residual tile ([128 x 64] SWIZZLE_128B boxes, zero fill past M) and its mask tile ([128 x BN/8] bytes, unswizzled;
+  // not loaded by the eval epilogue)
+  long long res_bytes() const { return (long long)sRes.size() + (p.eval ? 0 : (long long)sMask.size()); }
   void tma_load_res(int n0, int row0) {
     for (int r = 0; r < BM; r++)
       for (int c = 0; c < BN; c++) {
         const bool in = row0 + r < p.M;
         const uint16_t v = in ? p.R[(size_t)(row0 + r) * p.N + n0 + c] : 0;
         memcpy(sRes.data() + stage_elem_byte(c, r), &v, 2);
-        if (c % 8 == 0) sMask[mask_byte(BN, c, r)] = in ? p.mask[(size_t)(row0 + r) * (p.N / 8) + (n0 + c) / 8] : 0;
+        if (c % 8 == 0 && !p.eval) sMask[mask_byte(BN, c, r)] = in ? p.mask[(size_t)(row0 + r) * (p.N / 8) + (n0 + c) / 8] : 0;
       }
-    res_full.complete_tx((long long)sRes.size() + (long long)sMask.size());
+    res_full.complete_tx(res_bytes());
   }
   void release(int s) { for (int w = 0; w < kConsumerWarps / 2; w++) empty[s].arrive(); }   // lane 0 of each warp
 
@@ -171,7 +176,7 @@ struct CTA {
       }
       if (p.res) {
         res_empty.wait(rs.ph ^ 1u);
-        res_full.arrive_expect_tx((long long)sRes.size() + (long long)sMask.size());
+        res_full.arrive_expect_tx(res_bytes());
         tma_load_res(n0, m_blk * BM);
         rs.advance(1);
       }
@@ -183,6 +188,8 @@ struct CTA {
     const int num_k = p.K / BK, n0 = walk.n_blk * BN;
     std::vector<float> d((size_t)64 * BN);               // the warpgroup's accumulator fragments
     std::vector<float> s1(BN, 0.f), s2(BN, 0.f), shift(BN, 0.f);   // registers of the column owners t < BN
+    if (p.eval && wg == 0)                                 // a, b of the CTA's columns into the sums region
+      for (int t = 0; t < BN; t++) { sums[t] = p.a[n0 + t]; sums[BN + t] = p.b[n0 + t]; }
     Ring st, rs;
     for (int m_blk = walk.m_first; m_blk < walk.num_m; m_blk += walk.m_step) {
       int prev = 0;
@@ -206,7 +213,20 @@ struct CTA {
             for (int i = 0; i < 2; i++) {
               const int row = frag_row + 8 * i;
               float* v = &d[(size_t)(row - wg * 64) * BN + col];
-              if (p.res) {
+              if (p.eval) {
+                v[0] = std::fma(sums[col], v[0], sums[BN + col]);
+                v[1] = std::fma(sums[col + 1], v[1], sums[BN + col + 1]);
+                if (p.res) {
+                  uint16_t r2[2];
+                  memcpy(r2, sRes.data() + stage_elem_byte(col, row), 4);
+                  v[0] += bf2f(r2[0]);
+                  v[1] += bf2f(r2[1]);
+                }
+                if (p.relu) {
+                  v[0] = v[0] > 0.f ? v[0] : 0.f;
+                  v[1] = v[1] > 0.f ? v[1] : 0.f;
+                }
+              } else if (p.res) {
                 uint16_t r2[2];
                 memcpy(r2, sRes.data() + stage_elem_byte(col, row), 4);
                 const uint32_t bits = (uint32_t)sMask[mask_byte(BN, col, row)] >> (col & 7);
@@ -228,7 +248,7 @@ struct CTA {
         for (int b = 0; b < BN / 64; b++) tma_store(sOut.data() + (size_t)b * kBoxBytes, n0 + b * 64, m_blk * BM);
       }
       const int r_end = std::min(wg * 64 + 64, p.M - m_blk * BM);
-      for (int t = 0; t < BN && !p.res; t++) {             // col_owner
+      for (int t = 0; t < BN && !p.res && !p.eval; t++) {  // col_owner
         if (m_blk == walk.m_first) {
           uint16_t h;
           memcpy(&h, sOut.data() + stage_elem_byte(t, 0), 2);
@@ -246,10 +266,10 @@ struct CTA {
         s2[t] += t2;
       }
     }
-    if (wg == 1 && !p.res)
+    if (wg == 1 && !p.res && !p.eval)
       for (int t = 0; t < BN; t++) { sums[2 * t] = s1[t]; sums[2 * t + 1] = s2[t]; }
     cons.sync();
-    if (wg == 0 && !p.res && walk.m_first < walk.num_m)
+    if (wg == 0 && !p.res && !p.eval && walk.m_first < walk.num_m)
       for (int t = 0; t < BN; t++) {
         p.partials[partial_index(walk.m_first, p.N, n0 + t)] = s1[t] + sums[2 * t];
         p.partials[partial_index(walk.m_first, p.N, n0 + t) + 1] = s2[t] + sums[2 * t + 1];
@@ -263,9 +283,9 @@ struct CTA {
   }
 };
 
-static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mean = false) {
+static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mean = false, bool eval = false, bool relu = false) {
   Problem p;
-  p.M = M; p.N = N; p.K = K; p.BN = N % 128 == 0 ? 128 : 64; p.res = res;
+  p.M = M; p.N = N; p.K = K; p.BN = N % 128 == 0 ? 128 : 64; p.res = res; p.eval = eval; p.relu = relu;
   p.X.resize((size_t)M * K); p.W.resize((size_t)N * K); p.Y.assign((size_t)M * N, 0xffff);
   uint32_t x = 12345u + (uint32_t)M * 7u + (uint32_t)N * 13u + (uint32_t)K;
   auto rnd = [&] { x = x * 1664525u + 1013904223u; return ((int)(x >> 20) % 2001 - 1000) / 1000.0f; };
@@ -278,6 +298,10 @@ static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mea
     p.R.resize((size_t)M * N); p.mask.resize((size_t)M * N / 8);
     for (auto& v : p.R) v = f2bf(rnd());
     for (auto& v : p.mask) { x = x * 1664525u + 1013904223u; v = (uint8_t)(x >> 24); }
+  }
+  if (eval) {
+    p.a.resize(N); p.b.resize(N);
+    for (int n = 0; n < N; n++) { p.a[n] = 0.5f + rnd(); p.b[n] = rnd(); }
   }
   // launch geometry exactly as launch<BN>() in gemm_bnstats.cu
   const int num_n = N / p.BN, num_m = (M + BM - 1) / BM;
@@ -301,7 +325,12 @@ static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mea
     for (int n = 0; n < N; n++) {
       float acc = 0.f;
       for (int k = 0; k < K; k++) acc += bf2f(p.X[(size_t)m * K + k]) * bf2f(p.W[(size_t)n * K + k]);
-      if (res && ((p.mask[(size_t)m * (N / 8) + n / 8] >> (n % 8)) & 1)) acc += bf2f(p.R[(size_t)m * N + n]);
+      if (eval) {
+        acc = p.a[n] * acc + p.b[n] + (res ? bf2f(p.R[(size_t)m * N + n]) : 0.f);
+        if (relu && acc < 0.f) acc = 0.f;
+      } else if (res && ((p.mask[(size_t)m * (N / 8) + n / 8] >> (n % 8)) & 1)) {
+        acc += bf2f(p.R[(size_t)m * N + n]);
+      }
       const uint16_t want = f2bf(acc);
       const uint16_t got = p.Y[(size_t)m * N + n];
       if (std::fabs(bf2f(want) - bf2f(got)) > 1e-2f * std::fabs(bf2f(want)) + 1e-3f) bad++;   // summation order differs
@@ -313,7 +342,7 @@ static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mea
   long long covered = 0;
   for (int g = 0; g < groups; g++) covered += walk_rows(g, groups, M);
   if (covered != M) bad++;
-  for (int n = 0; n < N && !res; n++) {
+  for (int n = 0; n < N && !res && !eval; n++) {
     const double k0 = bf2f(p.Y[n]);
     const double want1 = rs1[n] - M * k0, want2 = rs2[n] - 2 * k0 * rs1[n] + M * k0 * k0;
     double s1 = 0, s2 = 0;
@@ -325,7 +354,8 @@ static int run_case(int M, int N, int K, int sms, bool res = false, bool big_mea
     }
     if (std::fabs(s1 - want1) > 1e-3 * (std::fabs(want1) + 1.0) || std::fabs(s2 - want2) > 1e-3 * (want2 + 1.0)) bad++;
   }
-  printf("M=%-5d N=%-4d K=%-4d BN=%-3d grid=%-3d groups=%-3d %s: %s\n", M, N, K, p.BN, grid, groups, res ? "dgrad+res " : "",
+  printf("M=%-5d N=%-4d K=%-4d BN=%-3d grid=%-3d groups=%-3d %s%s: %s\n", M, N, K, p.BN, grid, groups, eval ? "eval" : "",
+         res ? (eval ? "+res " : "dgrad+res ") : (eval ? " " : ""),
          bad ? "MISMATCH" : "ok");
   return bad;
 }
@@ -345,6 +375,14 @@ int main() {
   bad += run_case(2048, 256, 64, 4, true);
   bad += run_case(1000, 128, 320, 3, true);
   bad += run_case(700, 256, 192, 2, true);
+  // eval epilogue (BatchNorm with running statistics, residual loaded without a mask): the residual cases above, BN = 64 with
+  // and without residual, ragged M, with and without ReLU
+  bad += run_case(2048, 256, 64, 4, true, false, true, true);
+  bad += run_case(1000, 128, 320, 3, true, false, true, true);
+  bad += run_case(700, 256, 192, 2, true, false, true, false);
+  bad += run_case(700, 192, 192, 6, true, false, true, true);
+  bad += run_case(100, 64, 128, 4, false, false, true, true);
+  bad += run_case(1000, 128, 320, 3, false, false, true, false);
   bad += g_deadlocks.load();
   printf(bad ? "gemm_pipeline_model: FAILED (%d)\n" : "gemm_pipeline_model: all cases match the reference GEMM and column sums\n", bad);
   return bad ? 1 : 0;

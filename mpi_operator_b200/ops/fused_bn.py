@@ -2,10 +2,12 @@
 
 ``bn_act(bn_module, x, residual=None, relu=True)`` computes
 ``relu(batch_norm(x) [+ residual])`` with the module's parameters and running
-statistics. The fused kernels run when x is a CUDA bf16 channels-last tensor in
-training mode with a supported channel count; anything else (CPU, eval, fp32)
-takes the plain PyTorch path, so models stay runnable everywhere and
-``state_dict`` layout is untouched.
+statistics. The fused kernels run when x is a CUDA bf16 channels-last tensor with
+a supported channel count, in training mode, or in eval mode when the module uses
+its running statistics and no autograd graph is recorded (one kernel per layer,
+``b200mpi_bn_act_eval``); anything else (CPU, fp32, eval with autograd) takes the
+plain PyTorch path, so models stay runnable everywhere and ``state_dict`` layout
+is untouched.
 """
 from __future__ import annotations
 
@@ -32,6 +34,46 @@ def fused_bn_available(x: torch.Tensor, bn: torch.nn.BatchNorm2d) -> bool:
     if n * h * w < 2:
         return False
     return bool(_lib().b200mpi_bn_supported(n * h * w, c)) and x.is_contiguous(memory_format=torch.channels_last)
+
+
+def _eval_bn_ready(bn: torch.nn.BatchNorm2d, *inputs) -> bool:
+    """Eval mode with running statistics (PyTorch would use batch statistics otherwise) and nothing for autograd to record:
+    BatchNorm is a fixed per-channel affine map, which the eval kernels apply."""
+    if not (_ENABLED and not bn.training and bn.track_running_stats and bn.running_mean is not None
+            and bn.running_var is not None):
+        return False
+    params = (bn.weight, bn.bias)
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs + params):
+        return False
+    return all(t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+               for t in params + (bn.running_mean, bn.running_var))
+
+
+def _eval_input_ok(x: torch.Tensor, bn: torch.nn.BatchNorm2d) -> bool:
+    if not (x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[1] == bn.num_features
+            and x.is_contiguous(memory_format=torch.channels_last) and x.data_ptr() % 16 == 0):
+        return False
+    n, c, h, w = x.shape
+    return n * h * w >= 1 and bool(_lib().b200mpi_bn_supported(n * h * w, c))
+
+
+def _bn_eval(bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual, relu: bool) -> torch.Tensor:
+    n, c, h, w = x.shape
+    y = torch.empty_like(x, memory_format=torch.channels_last)
+    rc = _lib().b200mpi_bn_act_eval(x.data_ptr(), _ptr(residual), y.data_ptr(), _ptr(bn.weight), _ptr(bn.bias),
+                                    bn.running_mean.data_ptr(), bn.running_var.data_ptr(), n * h * w, c, bn.eps, int(relu),
+                                    torch.cuda.current_stream(x.device).cuda_stream)
+    if rc != 0:
+        raise RuntimeError(f"b200mpi_bn_act_eval failed ({rc})")
+    global _LAUNCHES
+    _LAUNCHES += 1
+    return y
+
+
+def _residual_cl(residual: torch.Tensor):
+    if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
+        residual = residual.contiguous(memory_format=torch.channels_last)
+    return residual
 
 
 _WS_CACHE = {}
@@ -147,6 +189,11 @@ class _BNAct(torch.autograd.Function):
 
 
 def bn_act(bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual: torch.Tensor = None, relu: bool = True) -> torch.Tensor:
+    if (_eval_bn_ready(bn, x, residual) and _eval_input_ok(x, bn)
+            and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape == x.shape))):
+        residual = _residual_cl(residual)
+        if residual is None or residual.data_ptr() % 16 == 0:
+            return _bn_eval(bn, x, residual, relu)
     if fused_bn_available(x, bn) and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape == x.shape)):
         if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
             residual = residual.contiguous(memory_format=torch.channels_last)
@@ -199,10 +246,14 @@ def _grad_key(t: torch.Tensor):
     return (t.data_ptr(), t._version, tuple(t.shape), t.stride(), t.dtype)
 
 
-def _conv1x1_eligible(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor) -> bool:
-    if not (conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.padding == (0, 0) and conv.dilation == (1, 1)
+def _conv1x1_geometry(conv: torch.nn.Conv2d, x: torch.Tensor) -> bool:
+    return (conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.padding == (0, 0) and conv.dilation == (1, 1)
             and conv.groups == 1 and conv.bias is None and x.is_cuda and x.dim() == 4 and x.dtype == torch.bfloat16
-            and x.is_contiguous(memory_format=torch.channels_last) and bn.training and bn.affine and bn.track_running_stats
+            and x.is_contiguous(memory_format=torch.channels_last))
+
+
+def _conv1x1_eligible(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor) -> bool:
+    if not (_conv1x1_geometry(conv, x) and bn.training and bn.affine and bn.track_running_stats
             and bn.momentum is not None and _ENABLED):
         return False
     from . import gemm_bnstats
@@ -317,6 +368,8 @@ def conv_bn_act(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor
                 relu: bool = True, link: ResidualLink = None) -> torch.Tensor:
     """``relu(bn(conv(x)) [+ residual])``. With B200MPI_FUSED_CONV1X1=1 an eligible 1x1 stride-1 convolution runs on the
     wgmma GEMM whose epilogue already produces the BatchNorm statistics; everything else is ``bn_act(bn, conv(x), ...)``.
+    In eval mode without autograd (``_eval_bn_ready``) the same GEMM applies the BatchNorm with its running statistics, the
+    residual and the ReLU in its epilogue instead: one kernel for the whole layer (M >= 128).
 
     ``link``: one ResidualLink per residual block whose residual is the input of its first 1x1 convolution, passed to both
     that call (``residual=None``: the link is armed if the fused dgrad can take the hand-over) and the call that adds the
@@ -324,8 +377,7 @@ def conv_bn_act(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor
     if (_CONV1X1 and _conv1x1_eligible(conv, bn, x)
             and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape[0] == x.shape[0]
                                       and residual.shape[1] == conv.out_channels and residual.shape[2:] == x.shape[2:]))):
-        if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
-            residual = residual.contiguous(memory_format=torch.channels_last)
+        residual = _residual_cl(residual)
         _count_batch(bn)
         w2d = conv.weight.to(torch.bfloat16).reshape(conv.out_channels, conv.in_channels)
         if link is not None and residual is None:
@@ -336,4 +388,18 @@ def conv_bn_act(conv: torch.nn.Conv2d, bn: torch.nn.BatchNorm2d, x: torch.Tensor
             link = None
         return _Conv1x1BNAct.apply(x, residual, w2d, bn.weight, bn.bias, bn.running_mean, bn.running_var, _ws(bn, x.device), bn.eps,
                                    bn.momentum, relu, getattr(bn, "_b200_grad_ready", None), link)
+    if _CONV1X1 and _conv1x1_geometry(conv, x) and _eval_bn_ready(bn, x, residual, conv.weight):
+        from . import gemm_bnstats
+        n, cin, h, w = x.shape
+        cout = conv.out_channels
+        if (gemm_bnstats.bn_eval_supported(n * h * w, cout, cin) and bn.num_features == cout and x.data_ptr() % 16 == 0
+                and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape == (n, cout, h, w)))):
+            residual = _residual_cl(residual)
+            res2d = residual.permute(0, 2, 3, 1).reshape(n * h * w, cout) if residual is not None else None
+            if res2d is None or res2d.data_ptr() % 16 == 0:
+                w2d = conv.weight.to(torch.bfloat16).reshape(cout, cin)
+                y = gemm_bnstats.gemm_bn_eval(x.permute(0, 2, 3, 1).reshape(n * h * w, cin), w2d, bn, res2d, relu)
+                global _LAUNCHES
+                _LAUNCHES += 1
+                return y.view(n, h, w, cout).permute(0, 3, 1, 2)
     return bn_act(bn, conv(x), residual=residual, relu=relu)

@@ -3,6 +3,7 @@
 
     y, partials, parts = gemm_bnstats_raw(x, weight)       # partial rows of plain sums
     y, partials, parts = gemm_bnstats_shifted(x, weight)   # the kernel's own rows, as BatchNorm merges them
+    y = gemm_bn_eval(x, weight, bn, residual, relu)        # eval mode: BatchNorm with running statistics in the epilogue
 
 ``x``: channels-last bf16 activations viewed as [M = N*H*W, Cin]; ``weight``: the convolution weight [Cout, Cin]
 (``conv.weight.view(Cout, Cin)``) in bf16. Both return the bf16 output [M, Cout] and ``parts`` rows of per-channel sums of
@@ -42,6 +43,9 @@ def lib() -> C.CDLL:
         L.b200mpi_gemm_bnstats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_longlong,
                                            C.c_int, C.c_int, C.c_void_p]
         L.b200mpi_gemm_dgrad_res_supported.argtypes = [C.c_longlong, C.c_int, C.c_int]
+        L.b200mpi_gemm_bn_eval_supported.argtypes = [C.c_longlong, C.c_int, C.c_int]
+        L.b200mpi_gemm_bn_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_float, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_void_p]
         L.b200mpi_gemm_dgrad_res.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_longlong, C.c_int, C.c_int, C.c_void_p]
         _lib = L
@@ -129,3 +133,37 @@ def dgrad_residual(dy: torch.Tensor, wt: torch.Tensor, r: torch.Tensor, mask: to
     if below is None:
         return dx
     return dx, partials[:parts.value * 2 * n].view(parts.value, n, 2), parts.value
+
+
+def bn_eval_supported(m: int, n: int, k: int) -> bool:
+    return bool(lib().b200mpi_gemm_bn_eval_supported(m, n, k))
+
+
+def gemm_bn_eval(x: torch.Tensor, weight: torch.Tensor, bn: torch.nn.BatchNorm2d, residual: torch.Tensor = None,
+                 relu: bool = True) -> torch.Tensor:
+    """``relu?(bn(x @ weight^T) [+ residual])`` with ``bn`` in eval mode, in one kernel: the epilogue applies
+    ``a = gamma * rsqrt(running_var + eps)``, ``b = beta - running_mean * a`` per column to the fp32 accumulator, adds the
+    residual and rounds to bf16 once. ``x`` [M,K], ``weight`` [N,K] and ``residual`` [M,N] are contiguous CUDA bf16; the
+    module's parameters and running statistics are fp32 and only read. Returns y [M,N] bf16."""
+    if not (x.is_cuda and x.dtype == weight.dtype == torch.bfloat16):
+        raise ValueError("gemm_bn_eval needs CUDA bf16 x and weight")
+    if x.dim() != 2 or weight.dim() != 2 or x.shape[1] != weight.shape[1] or not x.is_contiguous() or not weight.is_contiguous():
+        raise ValueError("expected contiguous x [M,K] and weight [N,K]")
+    m, k = x.shape
+    n = weight.shape[0]
+    if residual is not None and not (residual.dtype == torch.bfloat16 and residual.shape == (m, n) and residual.is_contiguous()):
+        raise ValueError("residual: contiguous bf16 [M,N]")
+    stats = [t for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var) if t is not None]
+    if (bn.running_mean is None or bn.running_var is None
+            or any(t.dtype != torch.float32 or t.numel() != n or not t.is_contiguous() or t.device != x.device for t in stats)):
+        raise ValueError("bn: fp32 contiguous parameters and running statistics of N channels on x's device")
+    if not bn_eval_supported(m, n, k):
+        raise ValueError(f"unsupported shape M={m} N={n} K={k} (M >= 128, N and K multiples of 64)")
+    y = torch.empty(m, n, dtype=torch.bfloat16, device=x.device)
+    p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    rc = lib().b200mpi_gemm_bn_eval(x.data_ptr(), weight.data_ptr(), y.data_ptr(), p(residual), p(bn.weight), p(bn.bias),
+                                    bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps), int(relu), m, n, k,
+                                    torch.cuda.current_stream(x.device).cuda_stream)
+    if rc != 0:
+        raise RuntimeError(f"b200mpi_gemm_bn_eval failed ({rc})")
+    return y

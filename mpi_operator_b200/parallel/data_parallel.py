@@ -309,6 +309,7 @@ class DataParallelTrainer:
             comm.add_stat_source(self._replayed_ops)
         self._folded_ops: list = []  # totals of graphs that were since re-captured
         self._fault = fault.injector(comm.rank)  # $B200MPI_FAULT recovery tests; disarmed when unset
+        self._eval_graphs: dict = {}    # evaluate() under cuda_graph: input shape -> (graph, static x, static y, stats, top-k)
         hooks = {}
         for b in self.state.buckets:
             for p in b.params:
@@ -596,29 +597,73 @@ class DataParallelTrainer:
             self.comm.host_barrier()
 
     # ---------------------------------------------------------- evaluation --
+    MAX_EVAL_GRAPHS = 2   # e.g. the full batch and a ragged last batch; further shapes run eagerly
+
+    def _eval_stats(self, x, y, topk):
+        """Eval-mode forward, loss and top-k hits packed into one vector ``[loss, hits@k / n ...]``; returns (vector, ks)."""
+        if self.autocast_dtype is not None:
+            with torch.autocast(self.device.type, dtype=self.autocast_dtype):
+                out = self.model(x)
+                loss = self.loss_fn(out, y)
+        else:
+            out = self.model(x)
+            loss = self.loss_fn(out, y)
+        ks = [k for k in topk if k <= out.shape[1]]
+        top = out.float().topk(max(ks), dim=1).indices if ks else None
+        stats = [loss.float().reshape(())] + [(top[:, :k] == y[:, None]).any(1).float().mean() for k in ks]
+        return torch.stack(stats).contiguous(), ks
+
+    def _eval_graph(self, x, y, topk):
+        """The eval graph for this input shape, captured on first use (at most MAX_EVAL_GRAPHS; None: run eagerly). Each has
+        its own static inputs and memory pool; replays read the live parameters and running statistics, which training updates
+        in place, so a graph stays valid across steps. Capture uses the eval kernels only: nothing the training step owns
+        (its graph, static buffers, BN workspace, running statistics) is written."""
+        key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, tuple(topk))
+        ent = self._eval_graphs.get(key)
+        if ent is not None or len(self._eval_graphs) >= self.MAX_EVAL_GRAPHS:
+            return ent
+        sx = torch.empty(x.shape, dtype=x.dtype, device=self.device)
+        if self.channels_last and x.dim() == 4:
+            sx = sx.contiguous(memory_format=torch.channels_last)
+        sy = torch.empty(y.shape, dtype=y.dtype, device=self.device)
+        sx.copy_(x)
+        sy.copy_(y)
+        s = torch.cuda.Stream(device=self.device)   # warm up eagerly first (cuDNN algorithm choice, allocator)
+        s.wait_stream(torch.cuda.current_stream(self.device))
+        with torch.cuda.stream(s):
+            self._eval_stats(sx, sy, topk)
+        torch.cuda.current_stream(self.device).wait_stream(s)
+        torch.cuda.synchronize(self.device)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, capture_error_mode="thread_local"):
+            vec, ks = self._eval_stats(sx, sy, topk)
+        ent = self._eval_graphs[key] = (g, sx, sy, vec, ks)
+        return ent
+
     @torch.no_grad()
     def evaluate(self, x, y, topk=(1, 5)):
         """Forward only, in eval mode (BatchNorm uses its running statistics), under the trainer's autocast setting; no gradient,
         no collective on the training path, the captured CUDA graph is left alone. Returns ``{"loss": ..., "top1": ..., "top5": ...,
-        "examples": n}`` averaged over the ranks (tf_cnn_benchmarks' ``--eval``: "Accuracy @ 1 / @ 5")."""
+        "examples": n}`` averaged over the ranks (tf_cnn_benchmarks' ``--eval``: "Accuracy @ 1 / @ 5").
+
+        With ``cuda_graph`` on CUDA the forward, loss and top-k run as one graph replay per call (one graph per input shape,
+        at most MAX_EVAL_GRAPHS); the average over the ranks stays an eager collective after it."""
         was_training = self.model.training
         self.model.eval()
         try:
-            x = x.to(self.device, non_blocking=True)
-            y = y.to(self.device, non_blocking=True)
-            if self.channels_last and x.dim() == 4:
-                x = x.contiguous(memory_format=torch.channels_last)
-            if self.autocast_dtype is not None:
-                with torch.autocast(self.device.type, dtype=self.autocast_dtype):
-                    out = self.model(x)
-                    loss = self.loss_fn(out, y)
+            ent = self._eval_graph(x, y, topk) if (self.use_graph and self._cuda) else None
+            if ent is not None:
+                g, sx, sy, out_vec, ks = ent
+                sx.copy_(x, non_blocking=True)
+                sy.copy_(y, non_blocking=True)
+                g.replay()
+                vec = out_vec.clone()
             else:
-                out = self.model(x)
-                loss = self.loss_fn(out, y)
-            ks = [k for k in topk if k <= out.shape[1]]
-            top = out.float().topk(max(ks), dim=1).indices if ks else None
-            stats = [loss.float().reshape(())] + [(top[:, :k] == y[:, None]).any(1).float().mean() for k in ks]
-            vec = torch.stack(stats).contiguous()
+                x = x.to(self.device, non_blocking=True)
+                y = y.to(self.device, non_blocking=True)
+                if self.channels_last and x.dim() == 4:
+                    x = x.contiguous(memory_format=torch.channels_last)
+                vec, ks = self._eval_stats(x, y, topk)
             if self.comm.world > 1:
                 self.comm.allreduce(vec, op="avg")
             vals = vec.tolist()

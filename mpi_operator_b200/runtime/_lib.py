@@ -101,6 +101,7 @@ def lib() -> C.CDLL:
     if hasattr(L, "b200mpi_bn_act_fwd_prestats"):
         L.b200mpi_bn_act_fwd_prestats.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i, C.c_longlong, i, f, f, i, vp]
     L.b200mpi_bn_act_bwd.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_longlong, i, i, vp]
+    L.b200mpi_bn_act_eval.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_longlong, i, f, i, vp]
     L.b200mpi_bn_act_bwd_prestats.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i, C.c_longlong, i, i, vp]
     L.b200mpi_set_tuning.argtypes = [vp, sz, sz, i, i]
     L.b200mpi_get_tuning.argtypes = [vp, C.POINTER(sz), C.POINTER(sz), C.POINTER(i), C.POINTER(i)]
