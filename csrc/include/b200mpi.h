@@ -176,6 +176,36 @@ int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t comm, int grad_win, size_t g
                                      float lr, float mu, float wd, int nesterov, int first_step,
                                      b200mpi_algo_t algo, void* stream,
                                      const uint8_t* group_map, const float* group_hyper, int num_groups);
+/* Same step with LARS (fp32 gradients): every parameter tensor q of the region
+ * whose table row has lars != 0 scales its update direction by the trust ratio
+ *   trust = eta*|w| / (|g| + wd*|w| + 1e-8)   (1 when |w| or |g| is 0)
+ *   d = trust*(g + wd*w); m = first_step ? d : mu*m + d; w -= lr*(nesterov ? d + mu*m : m)
+ * with g the averaged gradient and both norms over the whole tensor, before the
+ * update; other parameters get exactly the grouped SGD step. Two launches on
+ * `stream` (norms + board exchange, then the update); the gradient window is
+ * only read.
+ *   param_map    device [count/4] uint16: the parameter (0..num_params-1) of each
+ *                vector, non-decreasing; vectors past the last parameter hold
+ *                num_params.
+ *   param_table  device [num_params][2] uint8 {group (< num_groups), lars}.
+ *   group_hyper  device [num_groups][3] {lr, mu, wd}, read at run time.
+ *   board_win    symmetric window holding num_params*world*2 floats at board_off.
+ *   scratch      this rank's device scratch of scratch_bytes >=
+ *                b200mpi_lars_scratch_bytes(count, world, num_params), zero-filled
+ *                before its first use (the kernels leave it reusable).
+ *   trust_out    optional device [num_params] floats: the trust ratios of this
+ *                step (1 for non-LARS parameters).
+ * 1 <= num_params <= 1024. Emulated mode: momentum, scratch and trust_out are
+ * host arrays of world device pointers (trust_out may be NULL as a whole). */
+int b200mpi_allreduce_lars_sym(b200mpi_comm_t comm, int grad_win, size_t grad_off,
+                               int param_win, size_t param_off, int lowp_win, size_t lowp_off,
+                               void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale,
+                               int nesterov, int first_step, b200mpi_algo_t algo, void* stream,
+                               const float* group_hyper, int num_groups,
+                               const uint16_t* param_map, const uint8_t* param_table, int num_params,
+                               int board_win, size_t board_off, void* scratch, size_t scratch_bytes,
+                               float eta, void* trust_out);
+size_t b200mpi_lars_scratch_bytes(size_t count, int world, int num_params);
 size_t b200mpi_slice_elems(size_t count, int world, b200mpi_dtype_t dtype);
 /* Optional device-resident hyper-parameters {lr, momentum, weight_decay} (3 floats)
  * read by the fused kernels instead of the by-value arguments: a captured CUDA

@@ -106,6 +106,23 @@ constexpr int kAdaMaxBlocks = 64;                                   // CTAs per 
 constexpr size_t kAdaDotBytes = (size_t)96 << 10;                   // >= (kMaxRanks-1) pairs x kMaxRanks x kAdaMaxBlocks x 3 doubles
 static_assert((size_t)(kMaxRanks - 1) * kMaxRanks * kAdaMaxBlocks * 3 * sizeof(double) <= kAdaDotBytes, "dot board too small");
 cudaError_t launch_adasum(const Launch& l, const KArgs& a, int dtype);
+// Fused allreduce + LARS (lars.cu): fp32 gradients, the group table of the grouped SGD, two launches per bucket.
+constexpr int kLarsMaxParams = 1024;    // parameters per bucket (the trust ratios live in shared memory)
+constexpr float kLarsEps = 1e-8f;
+struct LarsArgs {
+  const uint16_t* pmap;           // bucket-local parameter of each fp32 vector, indexed like KArgs::buf; non-decreasing,
+                                  // bucket tails P
+  const uint8_t* ptab;            // [P][2] {group, lars} of each parameter
+  const float* ghyper;            // [G][3] {lr, mu, wd}
+  Win board;                      // [P][world] float2 {sum g^2, sum w^2} on every rank
+  char* scratch[kMaxRanks];       // per-rank scratch of lars_scratch_bytes (real mode: only [rank] is set)
+  float* trust_out[kMaxRanks];    // optional [P] trust ratios per rank
+  float eta;
+  int P;
+};
+size_t lars_scratch_bytes(size_t per, int P);
+cudaError_t launch_lars_norms(const Launch& l, const KArgs& a, const LarsArgs& L, int mode);
+cudaError_t launch_lars_update(const Launch& l, const KArgs& a, const LarsArgs& L, int mode);
 cudaError_t launch_scale_cast(cudaStream_t s, const void* in, int in_dt, void* out, int out_dt,
                               size_t count, float scale);
 cudaError_t launch_fill_u32(cudaStream_t s, uint32_t* p, uint32_t v, size_t n);

@@ -1174,6 +1174,66 @@ int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t c, int gwin, size_t goff, in
              });
 }
 
+size_t b200mpi_lars_scratch_bytes(size_t count, int world, int num_params) {
+  const size_t nvec = (count + 3) / 4;
+  return lars_scratch_bytes((nvec + world - 1) / world, num_params);
+}
+
+int b200mpi_allreduce_lars_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
+                               void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, int nesterov,
+                               int first_step, b200mpi_algo_t algo, void* stream, const float* group_hyper, int num_groups,
+                               const uint16_t* param_map, const uint8_t* param_table, int num_params, int bwin,
+                               size_t boff, void* scratch, size_t scratch_bytes, float eta, void* trust_out) {
+  if (gdtype != B200MPI_F32) return fail(B200MPI_ERR_INVALID, "allreduce_lars: LARS needs fp32 gradients");
+  if (!group_hyper || num_groups < 1 || num_groups > 256) return fail(B200MPI_ERR_INVALID, "allreduce_lars: a group table of 1 to 256 rows is required");
+  if (!param_map || !param_table) return fail(B200MPI_ERR_INVALID, "allreduce_lars: parameter map and parameter table must be given together");
+  if (num_params < 1 || num_params > kLarsMaxParams) return fail(B200MPI_ERR_INVALID, "allreduce_lars: num_params must be in [1, 1024]");
+  if (!scratch) return fail(B200MPI_ERR_INVALID, "allreduce_lars: scratch is required");
+  if (!(eta > 0.0f)) return fail(B200MPI_ERR_INVALID, "allreduce_lars: eta must be > 0");
+  if (count == 0) return 0;
+  auto okwin = [&](int w) { return w >= 0 && w < (int)c->wins.size() && c->wins[w].live; };
+  if (!okwin(gwin) || !okwin(pwin) || !okwin(bwin) || (lwin >= 0 && !okwin(lwin))) return fail(B200MPI_ERR_INVALID, "allreduce_lars: bad window");
+  if (count % 4 || goff % 16 || poff % 16 || boff % 16 || (lwin >= 0 && loff % 16)) return fail(B200MPI_ERR_INVALID, "allreduce_lars: count must be a multiple of the 16-byte vector and offsets 16-byte aligned");
+  if (goff + count * 4 > c->wins[gwin].bytes || poff + count * 4 > c->wins[pwin].bytes) return fail(B200MPI_ERR_INVALID, "allreduce_lars: region outside window");
+  if (boff + (size_t)num_params * c->world * 8 > c->wins[bwin].bytes) return fail(B200MPI_ERR_INVALID, "allreduce_lars: the norm board needs num_params * world * 8 bytes");
+  if (scratch_bytes < b200mpi_lars_scratch_bytes(count, c->world, num_params)) return fail(B200MPI_ERR_INVALID, "allreduce_lars: scratch smaller than b200mpi_lars_scratch_bytes");
+  int mode = MODE_P2P;
+  if (algo == B200MPI_ALGO_NVLS || (algo == B200MPI_ALGO_AUTO && c->multicast && count * 4 >= c->nvls_min && count * 4 > c->oneshot_max)) mode = MODE_NVLS;
+  if (mode == MODE_NVLS && !(c->multicast && c->wins[gwin].mc && c->wins[pwin].mc)) mode = MODE_P2P;
+  const size_t nvec = count / 4, per = (nvec + c->world - 1) / c->world;
+  int blocks = blocks_for(c, per, mode == MODE_NVLS ? 4 : 2, mode == MODE_NVLS ? c->nvls_blocks : c->max_blocks);
+  blocks = std::min(blocks, kMaxBlocks);                        // the scratch holds kMaxBlocks partial rows
+  if (c->local) blocks = std::min(blocks, emu_max_blocks(c));   // what run() launches: both kernels need the same grid
+  LarsArgs L;
+  memset(&L, 0, sizeof(L));
+  L.pmap = param_map; L.ptab = param_table; L.ghyper = group_hyper;
+  L.board = win_region(c, bwin, boff);
+  L.eta = eta; L.P = num_params;
+  const auto ranks = my_ranks(c);
+  std::vector<KArgs> args(c->local ? c->world : 1);
+  for (size_t k = 0; k < ranks.size(); k++) {
+    const int r = ranks[k];
+    KArgs& a = args[k];
+    memset(&a, 0, sizeof(a));
+    a.c = dev_comm(c, r);
+    a.buf = win_region(c, gwin, goff);
+    a.param = win_region(c, pwin, poff);
+    if (lwin >= 0) a.lowp = win_region(c, lwin, loff);
+    a.mom = reinterpret_cast<float*>(c->local ? reinterpret_cast<void* const*>(momentum)[r] : momentum);
+    a.nbytes = count * 4; a.nvec = nvec; a.per = per;
+    a.scale = scale; a.nesterov = nesterov; a.first_step = first_step;
+    L.scratch[r] = reinterpret_cast<char*>(c->local ? reinterpret_cast<void* const*>(scratch)[r] : scratch);
+    if (trust_out) L.trust_out[r] = reinterpret_cast<float*>(c->local ? reinterpret_cast<void* const*>(trust_out)[r] : trust_out);
+    if (!L.scratch[r] || ((uintptr_t)L.scratch[r] & 15)) return fail(B200MPI_ERR_INVALID, "allreduce_lars: scratch must be 16-byte aligned");
+  }
+  const int algo_used = mode == MODE_NVLS ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT;
+  int rc = run(c, (cudaStream_t)stream, blocks, "allreduce_lars", count * 4, algo_used, args,
+               [&](const Launch& l, const KArgs& a) { return launch_lars_norms(l, a, L, mode); });
+  if (rc) return rc;
+  return run(c, (cudaStream_t)stream, blocks, "lars_update", 0, algo_used, args,
+             [&](const Launch& l, const KArgs& a) { return launch_lars_update(l, a, L, mode); });
+}
+
 int b200mpi_set_hyper_ptr(b200mpi_comm_t c, const float* p) { c->hyper = p; return 0; }
 
 int b200mpi_broadcast_bytes(b200mpi_comm_t c, void* buf, size_t bytes, int root, void* stream) {

@@ -38,26 +38,30 @@ def _align(n: int, a: int) -> int:
 
 
 MAX_PARAM_GROUPS = 256   # the fused kernel's group map holds one byte per vector
-_GROUP_KEYS = {"params", "lr", "momentum", "weight_decay", "nesterov"}
+MAX_LARS_BUCKET_PARAMS = 1024   # the fused LARS kernels keep one trust ratio per parameter of a bucket in shared memory
+LARS_EPS = 1e-8                 # the fixed epsilon of the trust ratio's denominator (the kernels' kLarsEps)
+_GROUP_KEYS = {"params", "lr", "momentum", "weight_decay", "nesterov", "lars"}
 
 
 def _resolve_param_groups(model: nn.Module, param_groups: Optional[list], lr: float, momentum: float, weight_decay: float,
-                          nesterov: bool):
-    """torch-style ``param_groups`` -> (members, values): group 0 holds the trainable parameters no group lists, with the
-    trainer-level values; group k >= 1 is ``param_groups[k - 1]``, its missing keys taken from the trainer."""
+                          nesterov: bool, lars: bool = False):
+    """torch-style ``param_groups`` -> (members, values, lars flags): group 0 holds the trainable parameters no group lists,
+    with the trainer-level values; group k >= 1 is ``param_groups[k - 1]``, its missing keys taken from the trainer."""
     trainable = [p for p in model.parameters() if p.requires_grad]
     groups = list(param_groups or [])
     if len(groups) + 1 > MAX_PARAM_GROUPS:
         raise ValueError(f"{len(groups)} parameter groups: at most {MAX_PARAM_GROUPS - 1} besides the implicit group 0")
     known = {id(p) for p in trainable}
     taken = set()
-    members, values = [], [[lr, momentum, weight_decay]]
+    members, values, lars_flags = [], [[lr, momentum, weight_decay]], [bool(lars)]
     for k, g in enumerate(groups):
         if not isinstance(g, dict) or "params" not in g:
             raise ValueError(f"parameter group {k}: expected a dict with a 'params' entry")
         unknown = set(g) - _GROUP_KEYS
         if unknown:
-            raise ValueError(f"parameter group {k}: unsupported keys {sorted(unknown)} (lr, momentum, weight_decay)")
+            raise ValueError(f"parameter group {k}: unsupported keys {sorted(unknown)} (lr, momentum, weight_decay, lars)")
+        if "lars" in g and not isinstance(g["lars"], bool):
+            raise ValueError(f"parameter group {k}: 'lars' must be a bool, got {g['lars']!r}")
         if "nesterov" in g and bool(g["nesterov"]) != bool(nesterov):
             raise ValueError(f"parameter group {k}: nesterov is a trainer-wide setting ({nesterov}), not per group")
         ps = [g["params"]] if isinstance(g["params"], torch.Tensor) else list(g["params"])
@@ -69,8 +73,9 @@ def _resolve_param_groups(model: nn.Module, param_groups: Optional[list], lr: fl
             taken.add(id(p))
         members.append(ps)
         values.append([float(g.get("lr", lr)), float(g.get("momentum", momentum)), float(g.get("weight_decay", weight_decay))])
+        lars_flags.append(g.get("lars", bool(lars)))
     members.insert(0, [p for p in trainable if id(p) not in taken])
-    return members, values
+    return members, values, lars_flags
 
 
 @dataclass
@@ -81,6 +86,9 @@ class Bucket:
     params: List[nn.Parameter] = field(default_factory=list)
     pending: int = 0
     momentum: Optional[torch.Tensor] = None  # this rank's shard
+    lars: bool = False                       # holds a LARS parameter: runs the fused LARS kernels
+    param_table: Optional[torch.Tensor] = None   # [len(params), 2] uint8 {group, lars}, bucket-local parameter order
+    trust: Optional[torch.Tensor] = None     # LARS buckets: trust ratio of each parameter at the last synchronising step
 
 
 class FlatModelState:
@@ -95,9 +103,11 @@ class FlatModelState:
     bf16->fp32 gradient cast + accumulate: ~3 small kernels per layer disappear from the step."""
 
     def __init__(self, module: nn.Module, comm: Communicator, bucket_bytes: int = 32 << 20, bf16_params: bool = False,
-                 group_of: Optional[dict] = None):
+                 group_of: Optional[dict] = None, lars_of: Optional[dict] = None):
         """``group_of`` (parameter -> group index, missing: 0) builds ``group_map``: one uint8 group id per 4-element
-        vector of the flat buffers, which the grouped fused SGD kernel reads per vector."""
+        vector of the flat buffers, which the grouped fused SGD kernel reads per vector. ``lars_of`` (parameter -> bool,
+        missing: False) builds ``param_map`` and each bucket's ``{group, lars}`` parameter table for the fused LARS
+        kernels."""
         self.comm = comm
         self.bf16_params = bf16_params
         params = [p for p in module.parameters() if p.requires_grad]
@@ -179,6 +189,31 @@ class FlatModelState:
                 start = self.param_slot[p][1]
                 gmap[start // 4:(start + _align(p.numel(), pad)) // 4] = group_of.get(p, 0)
             self.group_map = gmap.to(self.flat_param.device)
+        self.param_map: Optional[torch.Tensor] = None
+        if lars_of is not None:
+            # bucket-local parameter index of each vector: a parameter's padding takes its index, the bucket tail the index
+            # one past the bucket's last parameter (the kernels' trust-1 dummy entry)
+            pmap = torch.zeros(self.total // 4, dtype=torch.int32)
+            for b in self.buckets:
+                pmap[b.start // 4:(b.start + b.numel) // 4] = len(b.params)
+                for k, p in enumerate(b.params):
+                    start = self.param_slot[p][1]
+                    pmap[start // 4:(start + _align(p.numel(), pad)) // 4] = k
+            self.param_map = pmap.to(torch.uint16).to(self.flat_param.device)
+            group_of = group_of or {}
+            for b in self.buckets:
+                b.lars = any(lars_of.get(p, False) for p in b.params)
+                if b.lars and len(b.params) > MAX_LARS_BUCKET_PARAMS:
+                    raise ValueError(f"bucket {b.index} holds {len(b.params)} parameters; the fused LARS kernels take at "
+                                     f"most {MAX_LARS_BUCKET_PARAMS} per bucket: use a smaller bucket_bytes")
+                b.param_table = torch.tensor([[group_of.get(p, 0), int(bool(lars_of.get(p, False)))] for p in b.params],
+                                             dtype=torch.uint8).to(self.flat_param.device)
+                if b.lars:
+                    b.trust = torch.ones(len(b.params), dtype=torch.float32, device=self.flat_param.device)
+
+    def bucket_param_map(self, b: Bucket) -> torch.Tensor:
+        """The slice of ``param_map`` covering bucket ``b``."""
+        return self.param_map[b.start // 4:(b.start + b.numel) // 4]
 
     def bucket_group_map(self, b: Bucket) -> torch.Tensor:
         """The slice of ``group_map`` covering bucket ``b`` (``b.start`` and ``b.numel`` are multiples of 8 elements)."""
@@ -243,6 +278,21 @@ class DataParallelTrainer:
     parameters in no group form group 0 with the trainer-level values, so the groups given are 1, 2, ... in
     ``trainer.param_groups`` and ``set_lr(lr, group=k)``. All three optimizer paths (fused kernel, ``fused_optimizer=False``,
     ``comm_backend="nccl"``) apply the same per-group update.
+
+    ``lars=True`` turns on LARS (You et al., 2017) for group 0 and is the default of groups without a ``"lars"`` key; the
+    MLPerf ResNet recipe leaves BatchNorm and biases out of it and out of weight decay::
+
+        no_lars = [p for p in model.parameters() if p.dim() == 1]
+        trainer = DataParallelTrainer(model, loss_fn, comm, lr=..., momentum=0.9, weight_decay=5e-5,
+                                      lars=True, trust_coefficient=0.001,
+                                      param_groups=[{"params": no_lars, "weight_decay": 0.0, "lars": False}])
+
+    At each synchronising step every parameter tensor ``w`` of a LARS group, with ``g`` its world-averaged gradient and both
+    norms taken over the fp32 master before the update, gets ``trust = eta * |w| / (|g| + wd * |w| + 1e-8)`` (``trust = 1``
+    when ``|w|`` or ``|g|`` is 0), ``d = trust * (g + wd * w)``, ``m = mu * m + d`` and ``w -= lr * (d + mu * m if nesterov
+    else m)``; other parameters keep the plain update (``trust = 1``). ``eta`` is ``trust_coefficient``, trainer-wide and
+    fixed at construction. Apex's ``LARC(clip=False)`` differs only where a norm is 0: it then also drops the weight decay.
+    ``lars_trust_ratios()`` returns the trust ratios of the last synchronising step.
     """
 
     def __init__(self, model: nn.Module, loss_fn: Callable, comm: Communicator, *, lr: float, momentum: float = 0.9,
@@ -250,7 +300,13 @@ class DataParallelTrainer:
                  autocast_dtype: Optional[torch.dtype] = torch.bfloat16, channels_last: bool = True,
                  cuda_graph: bool = True, fused_optimizer: bool = True, algo: Optional[str] = None,
                  comm_backend: str = "b200mpi", bf16_params: Optional[bool] = None, async_h2d: Optional[bool] = None,
-                 param_groups: Optional[list] = None):
+                 param_groups: Optional[list] = None, lars: bool = False, trust_coefficient: float = 0.001):
+        if not isinstance(lars, bool):
+            raise ValueError(f"lars must be a bool, got {lars!r}")
+        if not (isinstance(trust_coefficient, (int, float)) and float(trust_coefficient) > 0
+                and float(trust_coefficient) != float("inf")):
+            raise ValueError(f"trust_coefficient must be a finite number > 0, got {trust_coefficient!r}")
+        self.trust_coefficient = float(trust_coefficient)
         self.comm = comm
         self.device = torch.device("cuda", comm.device) if comm.device != "cpu" else torch.device("cpu")
         self._cuda = self.device.type == "cuda"
@@ -275,18 +331,27 @@ class DataParallelTrainer:
         bucket_bytes = bucket_bytes or int(os.environ.get("B200MPI_BUCKET_BYTES", 32 << 20))
         names = {p: n for n, p in model.named_parameters()}
         self._has_groups = param_groups is not None
-        members, values = _resolve_param_groups(model, param_groups, lr, momentum, weight_decay, nesterov)
+        members, values, lars_flags = _resolve_param_groups(model, param_groups, lr, momentum, weight_decay, nesterov, lars)
         self._group_names = [[names[p] for p in ps] for ps in members]
         self._group_vals = values        # host copy of group_hyper, [[lr, momentum, weight_decay], ...]
-        group_of = {p: k for k, ps in enumerate(members) for p in ps} if self._has_groups else None
-        self.state = FlatModelState(model, comm, bucket_bytes, bf16_params=self.bf16_params, group_of=group_of)
+        self._group_lars = lars_flags    # per group: LARS on or off
+        # LARS reads {lr, momentum, weight_decay} from the group table even without param_groups (one row)
+        self._lars = any(lars_flags)
+        self._tabled = self._has_groups or self._lars
+        group_of = {p: k for k, ps in enumerate(members) for p in ps} if self._tabled else None
+        lars_of = {p: lars_flags[k] for k, ps in enumerate(members) for p in ps} if self._lars else None
+        self.state = FlatModelState(model, comm, bucket_bytes, bf16_params=self.bf16_params, group_of=group_of,
+                                    lars_of=lars_of)
         self.state.broadcast_parameters(0)
         # {lr, momentum, weight_decay} on the device: graph replays follow schedules
         self.hyper = torch.tensor([lr, momentum, weight_decay], device=self.device, dtype=torch.float32)
         comm.set_hyper(self.hyper)
         self._lr, self._mu, self._wd = lr, momentum, weight_decay
         # with param_groups: one {lr, momentum, weight_decay} row per group on the device, read by the kernels the same way
-        self.group_hyper = torch.tensor(values, device=self.device, dtype=torch.float32) if self._has_groups else None
+        self.group_hyper = torch.tensor(values, device=self.device, dtype=torch.float32) if self._tabled else None
+        self._lars_board = self._lars_scratch = None
+        if self._lars:
+            self._alloc_lars()
         self.comm_stream = torch.cuda.Stream(device=self.device, priority=-1) if self._cuda else None
         self._graph: Optional[torch.cuda.CUDAGraph] = None
         self._static_x = self._static_y = None
@@ -349,10 +414,33 @@ class DataParallelTrainer:
 
     @property
     def param_groups(self) -> list:
-        """``[{"params": [parameter names], "lr": ..., "momentum": ..., "weight_decay": ...}, ...]``, group 0 (parameters
-        in no given group, trainer-level values) first. A copy: change values with ``set_lr``."""
-        return [{"params": list(n), "lr": v[0], "momentum": v[1], "weight_decay": v[2]}
-                for n, v in zip(self._group_names, self._group_vals)]
+        """``[{"params": [parameter names], "lr": ..., "momentum": ..., "weight_decay": ..., "lars": ...}, ...]``, group 0
+        (parameters in no given group, trainer-level values) first. A copy: change values with ``set_lr``."""
+        return [{"params": list(n), "lr": v[0], "momentum": v[1], "weight_decay": v[2], "lars": f}
+                for n, v, f in zip(self._group_names, self._group_vals, self._group_lars)]
+
+    def _alloc_lars(self) -> None:
+        """Norm board (a symmetric window of [P][world] float pairs) and per-rank scratch of the fused LARS kernels, sized
+        for the largest LARS bucket; one of each serves every bucket, as the buckets run in stream order."""
+        st = self.state
+        lb = [b for b in st.buckets if b.lars]
+        if not (self.fused and lb) or self._lars_board is not None:
+            return
+        P = max(len(b.params) for b in lb)
+        self._lars_board = self.comm.alloc_window(_align(P * self.comm.world * 8, 16))
+        nbytes = max(self.comm.lars_scratch_bytes(b.numel, len(b.params)) for b in lb)
+        self._lars_scratch = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+
+    def lars_trust_ratios(self) -> dict:
+        """``{parameter name: trust ratio}`` of every LARS parameter at the last synchronising step (1.0 before the first).
+        Reading it synchronises with the device."""
+        names = {p: n for n, p in self.model.named_parameters()}
+        out = {}
+        for b in self.state.buckets:
+            if b.lars:
+                vals, flags = b.trust.tolist(), b.param_table[:, 1].tolist()
+                out.update({names[p]: v for p, v, f in zip(b.params, vals, flags) if f})
+        return out
 
     @property
     def launches_per_step(self) -> int:
@@ -415,6 +503,14 @@ class DataParallelTrainer:
             g = st.flat_grad[b.start:b.start + b.numel]
             if self.comm.world > 1:
                 self._dist.all_reduce(g, op=self._dist.ReduceOp.AVG)
+        elif self.fused and b.lars:
+            self.comm.allreduce_lars_window(st.grad_win, b.start * 4, st.param_win, b.start * 4, b.momentum, b.numel,
+                                            torch.float32, group_hyper=self.group_hyper,
+                                            param_map=st.bucket_param_map(b), param_table=b.param_table,
+                                            board_win=self._lars_board, board_off=0, scratch=self._lars_scratch,
+                                            trust_coefficient=self.trust_coefficient, nesterov=self.nesterov,
+                                            lowp_win=st.lowp_win, lowp_off=b.start * 2, algo=self.algo,
+                                            stream=self.comm_stream, trust_out=b.trust)
         elif self.fused and self._has_groups:
             self.comm.allreduce_sgd_window(st.grad_win, b.start * 4, st.param_win, b.start * 4, b.momentum,
                                            b.numel, torch.float32, lr=self._lr, momentum_coef=self._mu,
@@ -437,7 +533,7 @@ class DataParallelTrainer:
         st = self.state
         if not hasattr(self, "_flat_mom"):
             self._flat_mom = torch.zeros_like(st.flat_param)
-        if self._has_groups:
+        if self._tabled:
             # the fused kernel's per-vector update: each 4-element vector takes its group's row of the table
             if not hasattr(self, "_group_index"):
                 self._group_index = st.group_map.long()
@@ -445,6 +541,8 @@ class DataParallelTrainer:
             lr, mu, wd = h[:, 0:1], h[:, 1:2], h[:, 2:3]
             p, m = st.flat_param.view(-1, 4), self._flat_mom.view(-1, 4)
             g = st.flat_grad.view(-1, 4) + wd * p
+            if self._lars:
+                g = g * self._unfused_trust()
             m.mul_(mu).add_(g)
             p.sub_(lr * (g + mu * m if self.nesterov else m))
             st.refresh_lowp()
@@ -456,6 +554,41 @@ class DataParallelTrainer:
         upd = g.add(self._flat_mom, alpha=self._mu) if self.nesterov else self._flat_mom
         st.flat_param.sub_(upd * self.hyper[0])
         st.refresh_lowp()
+
+    def _unfused_trust(self) -> torch.Tensor:
+        """LARS trust ratio of every 4-element vector of the flat buffers ([total / 4, 1]; 1 outside LARS parameters), from
+        the averaged gradients and the masters before the update; also stored as each bucket's ``trust``."""
+        st = self.state
+        if not hasattr(self, "_lars_index"):
+            # vector -> row of the parameter list below; bucket tails the trailing row, which holds trust 1
+            lp = [p for b in st.buckets for p in b.params]
+            self._lars_params = lp
+            self._lars_rows = {p: k for k, p in enumerate(lp)}
+            idx = torch.full((st.total // 4,), len(lp), dtype=torch.long)
+            pmap = st.param_map.cpu().long()
+            for b in st.buckets:
+                sl = slice(b.start // 4, (b.start + b.numel) // 4)
+                first = self._lars_rows[b.params[0]]
+                local = pmap[sl]
+                idx[sl] = torch.where(local < len(b.params), local + first, torch.full_like(local, len(lp)))
+            self._lars_index = idx.to(st.flat_param.device)
+            self._lars_flag = torch.tensor([bool(b.param_table[k, 1]) for b in st.buckets for k in range(len(b.params))],
+                                           device=st.flat_param.device)
+            self._lars_group = torch.tensor([int(b.param_table[k, 0]) for b in st.buckets for k in range(len(b.params))],
+                                            device=st.flat_param.device, dtype=torch.long)
+        lp = self._lars_params
+        views = [(st.param_slot[p][1], p.numel()) for p in lp]
+        wn = torch.stack(torch._foreach_norm([st.flat_param[s:s + n] for s, n in views]))
+        gn = torch.stack(torch._foreach_norm([st.flat_grad[s:s + n] for s, n in views]))
+        wd = self.group_hyper[self._lars_group, 2]
+        trust = torch.where(self._lars_flag & (wn > 0) & (gn > 0),
+                            self.trust_coefficient * wn / (gn + wd * wn + LARS_EPS), torch.ones_like(wn))
+        k = 0
+        for b in st.buckets:
+            if b.lars:
+                b.trust.copy_(trust[k:k + len(b.params)])
+            k += len(b.params)
+        return torch.cat([trust, trust.new_ones(1)])[self._lars_index].unsqueeze(1)
 
     # ----------------------------------------------------------- step --
     def _fwd_bwd(self, x, y):
@@ -708,7 +841,8 @@ class DataParallelTrainer:
         sd = {"format": "b200mpi.DataParallelTrainer/1", "model": masters, "momentum": momentum,
               "buffers": {n: b.detach().cpu().clone() for n, b in self.model.named_buffers()},
               "hyper": {"lr": float(self.hyper[0]), "momentum": float(self.hyper[1]), "weight_decay": float(self.hyper[2]),
-                        "nesterov": bool(self.nesterov)},
+                        "nesterov": bool(self.nesterov), "lars": bool(self._group_lars[0]),
+                        "trust_coefficient": self.trust_coefficient},
               "world_size_at_save": int(self.comm.world)}
         if self._has_groups:
             sd["param_groups"] = self.param_groups
@@ -718,7 +852,9 @@ class DataParallelTrainer:
         """Restore ``state_dict()`` output in a trainer built on the same model class (any world size, with or without the bf16
         shadow / fused optimizer). Not collective: every rank loads the same dictionary and keeps its own momentum shard.
         With ``load_hyper``, per-group values are restored when the checkpoint's parameter groups have the same members (by
-        name) as this trainer's; a checkpoint with groups into a trainer without them, or the reverse, is a ``ValueError``."""
+        name) as this trainer's; a checkpoint with groups into a trainer without them, or the reverse, is a ``ValueError``.
+        Which groups use LARS and ``trust_coefficient`` stay as this trainer was built (the checkpoint records them): the
+        momentum is the same state for SGD and LARS, so SGD and LARS checkpoints load into each other."""
         if sd.get("format") != "b200mpi.DataParallelTrainer/1":
             raise ValueError("not a DataParallelTrainer checkpoint")
         if load_hyper and ("param_groups" in sd) != self._has_groups:
@@ -763,6 +899,8 @@ class DataParallelTrainer:
             self._lr, self._mu, self._wd = h["lr"], h["momentum"], h["weight_decay"]
             self.hyper.copy_(torch.tensor([self._lr, self._mu, self._wd], dtype=torch.float32))
             self._group_vals[0] = [self._lr, self._mu, self._wd]
+            if self.group_hyper is not None and not self._has_groups:   # LARS without param_groups: its one-row table
+                self.group_hyper[0].copy_(self.hyper)
             if self._has_groups:
                 self._group_vals = [[g["lr"], g["momentum"], g["weight_decay"]] for g in sd["param_groups"]]
                 self.group_hyper.copy_(torch.tensor(self._group_vals, dtype=torch.float32))

@@ -363,6 +363,55 @@ class Communicator:
             count, dtype_code(grad_dtype), s, lr, momentum_coef, weight_decay, int(nesterov), int(first_step),
             resolve_algo(algo), _stream_ptr(stream)), "allreduce_sgd_sym")
 
+    def lars_scratch_bytes(self, count: int, num_params: int) -> int:
+        """Bytes of the per-rank scratch ``allreduce_lars_window`` needs for a region of ``count`` fp32 elements."""
+        return int(_lib.lib().b200mpi_lars_scratch_bytes(count, self.world, num_params))
+
+    def allreduce_lars_window(self, grad_win: Window, grad_off: int, param_win: Window, param_off: int, momentum,
+                              count: int, grad_dtype, *, group_hyper, param_map, param_table, board_win: Window,
+                              board_off: int, scratch, trust_coefficient: float, nesterov: bool = False,
+                              first_step: bool = False, scale: Optional[float] = None, lowp_win: Optional[Window] = None,
+                              lowp_off: int = 0, algo=None, stream=None, trust_out=None) -> None:
+        """Fused gradient-average + LARS step; see b200mpi_allreduce_lars_sym. Two launches on ``stream``.
+
+        ``param_map`` is a CUDA uint16 tensor of ``count // 4`` entries, the bucket-local parameter of each 4-element vector
+        (non-decreasing; vectors past the last parameter hold ``P``), ``param_table`` a contiguous CUDA uint8 ``[P, 2]``
+        tensor of ``{group, lars}`` rows and ``group_hyper`` the ``[G, 3]`` table of ``allreduce_sgd_window``. ``board_win``
+        holds ``P * world`` float pairs at ``board_off``. ``scratch`` is this rank's zero-filled CUDA uint8 tensor of at
+        least ``lars_scratch_bytes(count, P)`` bytes and ``trust_out`` an optional float32 ``[P]`` tensor that receives the
+        trust ratios (on an emulated communicator: lists of ``world`` tensors, one per rank)."""
+        torch = _torch()
+        if grad_dtype != torch.float32:
+            raise B200MPIError("allreduce_lars_window: LARS needs float32 gradients")
+        dev = torch.device("cuda", self.device)
+        if not (param_map.device == dev and param_map.dtype == torch.uint16 and param_map.is_contiguous()
+                and param_map.numel() == count // 4):
+            raise B200MPIError(f"allreduce_lars_window: param_map must be a contiguous uint16 tensor of {count // 4} entries on {dev}")
+        if not (param_table.device == dev and param_table.dtype == torch.uint8 and param_table.is_contiguous()
+                and param_table.dim() == 2 and param_table.shape[1] == 2 and param_table.shape[0] >= 1):
+            raise B200MPIError(f"allreduce_lars_window: param_table must be a contiguous uint8 [P, 2] tensor on {dev}")
+        if not (group_hyper.device == dev and group_hyper.dtype == torch.float32 and group_hyper.is_contiguous()
+                and group_hyper.dim() == 2 and group_hyper.shape[1] == 3 and 1 <= group_hyper.shape[0] <= 256):
+            raise B200MPIError(f"allreduce_lars_window: group_hyper must be a contiguous float32 [G, 3] tensor on {dev}, 1 <= G <= 256")
+        P = int(param_table.shape[0])
+        scr = scratch if isinstance(scratch, (list, tuple)) else [scratch]
+        if any(not (s.device == dev and s.dtype == torch.uint8 and s.is_contiguous()) for s in scr):
+            raise B200MPIError(f"allreduce_lars_window: scratch must be contiguous uint8 tensors on {dev}")
+        if trust_out is not None:
+            outs = trust_out if isinstance(trust_out, (list, tuple)) else [trust_out]
+            if any(not (t.device == dev and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == P) for t in outs):
+                raise B200MPIError(f"allreduce_lars_window: trust_out must be contiguous float32 tensors of {P} entries on {dev}")
+        pm, _ = self._ptrs(momentum)
+        ps, _ = self._ptrs(scratch)
+        pt = self._ptrs(trust_out)[0] if trust_out is not None else None
+        s = (1.0 / self.world) if scale is None else float(scale)
+        check(_lib.lib().b200mpi_allreduce_lars_sym(
+            self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm, count,
+            dtype_code(grad_dtype), s, int(nesterov), int(first_step), resolve_algo(algo), _stream_ptr(stream),
+            group_hyper.data_ptr(), int(group_hyper.shape[0]), param_map.data_ptr(), param_table.data_ptr(), P,
+            board_win.id, board_off, ps, min(t.numel() for t in scr), float(trust_coefficient), pt),
+            "allreduce_lars_sym")
+
     # ------------------------------------------------------ point-to-point --
     @property
     def has_p2p(self) -> bool:
