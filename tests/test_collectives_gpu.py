@@ -8,7 +8,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module", params=[2, 4, 8])
+@pytest.fixture(scope="module", params=list(range(1, 9)))
 def comm(request):
     from mpi_operator_b200.runtime.comm import Communicator
     c = Communicator.local(request.param, device=0)
@@ -68,7 +68,8 @@ def test_allreduce_pipelined_user_pointers(comm, dtype, n, chunk):
             for o in outs:
                 torch.testing.assert_close(o.float(), want.to(dtype).float(), rtol=rtol, atol=atol)
                 assert torch.equal(o, outs[0])
-        assert any(o["op"] == "allreduce_pipe" for o in comm.stats(native_only=True)["ops"])
+        if comm.world > 1:   # a single rank has nothing to pipeline: the staged kernel runs
+            assert any(o["op"] == "allreduce_pipe" for o in comm.stats(native_only=True)["ops"])
     finally:
         comm.set_pipe(min_bytes=8 << 20, chunk_bytes=1 << 20, depth=3)
 
@@ -103,7 +104,8 @@ def test_pipelined_allgather_reduce_scatter_broadcast(comm, n, chunk):
             for b in bs:
                 assert torch.equal(b, bwant)
         names = {o["op"] for o in comm.stats(native_only=True)["ops"]}
-        assert {"allgather_pipe", "reduce_scatter_pipe", "broadcast_pipe"} <= names
+        if comm.world > 1:
+            assert {"allgather_pipe", "reduce_scatter_pipe", "broadcast_pipe"} <= names
     finally:
         comm.set_pipe(min_bytes=8 << 20, chunk_bytes=1 << 20, depth=3)
 

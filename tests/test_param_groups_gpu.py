@@ -20,7 +20,7 @@ def _real_comm(tag):
     return Communicator.create(0, 1, 0, f"t-groups-{tag}-{os.getpid()}")
 
 
-@pytest.fixture(scope="module", params=["real1", 2, 4, 8])
+@pytest.fixture(scope="module", params=["real1", 2, 3, 4, 6, 8])
 def comm(request):
     from mpi_operator_b200.runtime.comm import Communicator
     c = _real_comm("k") if request.param == "real1" else Communicator.local(request.param, device=0)
