@@ -116,11 +116,14 @@ def test_bn_eval_kernel_matches_fp64(c):
 
 
 # --------------------------------------------------------------------------------------------- GEMM eval epilogue --
-# (M, K = Cin, N = Cout) of ResNet-101's stride-1 1x1 convolutions at batch 64, a ragged M and a single row tile
+# (M, K = Cin, N = Cout) of ResNet-101's stride-1 1x1 convolutions at batch 64, a ragged M and a single row tile; then
+# tile width 64 with several column blocks, 3 and 5 k-blocks, one CTA per column block (N = 8384: 131 blocks of 64) and
+# fewer row tiles than m-groups (M = 129, 255)
 GEMM_SHAPES = [(64 * 56 * 56, 64, 64), (64 * 56 * 56, 64, 256), (64 * 56 * 56, 256, 64), (64 * 28 * 28, 256, 128),
                (64 * 28 * 28, 128, 512), (64 * 28 * 28, 512, 128), (64 * 14 * 14, 512, 256), (64 * 14 * 14, 256, 1024),
                (64 * 14 * 14, 1024, 256), (64 * 7 * 7, 1024, 512), (64 * 7 * 7, 512, 2048), (64 * 7 * 7, 2048, 512),
-               (1000, 256, 128), (1000, 64, 64), (128, 512, 2048)]
+               (1000, 256, 128), (1000, 64, 64), (128, 512, 2048),
+               (129, 192, 192), (255, 320, 320), (1000, 128, 8384), (256, 2048, 192), (1000, 4096, 256)]
 
 GEMM_CASE = r"""
 M, K, N = {m}, {k}, {n}
