@@ -25,8 +25,15 @@
 // slot per (pair, source rank, source CTA) and every slot a launch reads was written in that launch, so nothing has to be
 // zeroed between launches. All CTAs of a launch must be co-resident (spin barriers): the host caps the grid at kAdaMaxBlocks.
 //
-// Status: numerics test (8 / 4 / 2 virtual ranks against the fp64 tree) in tests/test_zzz_adasum_gpu.py, which sorts last
-// in the GPU tier. hvd/adasum.py uses it only with B200MPI_ADASUM_KERNEL=1.
+// Arithmetic (the same contract as hvd/adasum.py: adasum_pair; tests/adasum_oracle.py states its one correct output):
+//   * inputs are widened to fp32 (exact for bf16 / f16); the products a.b, a.a and b.b are formed in fp64, where an
+//     fp32 x fp32 product is exact, and summed in fp64 (per-thread chain, warp butterfly, warps, then the board);
+//   * coefficient c = (float)(1.0 - d / (2.0 * n)) when n > 0, else 1.0f - no clamp, so scale never enters it;
+//   * combine z = fl32(fl32(ca x) + fl32(cb y)), written with __fmul_rn / __fadd_rn so that nvcc cannot contract it into
+//     an FFMA (which operand got fused would be the compiler's choice, and no oracle could state the bits);
+//   * intermediate levels stay fp32 in W; the last level rounds once, to nearest even, into T.
+// Only the order of the fp64 sums depends on the grid. The coefficients are exact up to that order, so a test whose
+// coefficients sit away from an fp32 rounding midpoint has exactly one correct output whatever the CTA count.
 #include "kernels.h"
 
 namespace b200mpi {
@@ -100,10 +107,15 @@ __device__ __forceinline__ void block_sums(double* vals, int n, double (*warp_pa
 
 template <int VN>
 __device__ __forceinline__ void dots3(double* acc, const float* x, const float* y) {
-  float d = 0.f, nx = 0.f, ny = 0.f;
 #pragma unroll
-  for (int j = 0; j < VN; j++) { d = fmaf(x[j], y[j], d); nx = fmaf(x[j], x[j], nx); ny = fmaf(y[j], y[j], ny); }
-  acc[0] += (double)d; acc[1] += (double)nx; acc[2] += (double)ny;
+  for (int j = 0; j < VN; j++) {   // fp64 products of fp32 values are exact: one rounding per add, none per product
+    const double xd = x[j], yd = y[j];
+    acc[0] = fma(xd, yd, acc[0]); acc[1] = fma(xd, xd, acc[1]); acc[2] = fma(yd, yd, acc[2]);
+  }
+}
+
+__device__ __forceinline__ float combine(float ca, float x, float cb, float y) {
+  return __fadd_rn(__fmul_rn(ca, x), __fmul_rn(cb, y));   // no FFMA: each product is rounded to fp32 on its own
 }
 
 template <typename T>
@@ -215,8 +227,8 @@ k_adasum(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu) {
 #pragma unroll
           for (int j = 0; j < V4; j++) {
             const float4 x = W[g * wq + i * V4 + j], y = W[h * wq + i * V4 + j];
-            z[4 * j] = ca * x.x + cb * y.x; z[4 * j + 1] = ca * x.y + cb * y.y;
-            z[4 * j + 2] = ca * x.z + cb * y.z; z[4 * j + 3] = ca * x.w + cb * y.w;
+            z[4 * j] = combine(ca, x.x, cb, y.x); z[4 * j + 1] = combine(ca, x.y, cb, y.y);
+            z[4 * j + 2] = combine(ca, x.z, cb, y.z); z[4 * j + 3] = combine(ca, x.w, cb, y.w);
           }
           if (last) {
             const uint4 o = VecTraits<T>::pack(z);

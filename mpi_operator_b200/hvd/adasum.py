@@ -7,9 +7,20 @@ ranks: orthogonal gradients add, parallel gradients average. Two device paths:
 * ``B200MPI_ADASUM_KERNEL=1``: ``Communicator.adasum`` - ONE kernel per tensor (csrc/kernels/adasum.cu), each rank owns
   one slice of every vector, the tree levels run inside the launch over NVSwitch peer memory (S bytes pulled + S bytes
   pushed per rank, log2(N)+2 flag barriers). Power-of-two worlds, f32 / bf16 / f16, tensors up to
-  ``Communicator.adasum_max_bytes``. Opt-in (tests/test_zzz_adasum_gpu.py is its numerics test).
-* otherwise every rank gathers the N tensors (one b200mpi allgather kernel) and folds the tree locally in fp32 -
-  identical bits on all ranks, O(N*S) scratch; fine for the example-scale models that use Adasum.
+  ``Communicator.adasum_max_bytes``. Opt-in.
+* otherwise every rank gathers the N tensors (one b200mpi allgather kernel) and folds the tree locally with
+  ``adasum_tree`` - identical bits on all ranks, O(N*S) scratch; fine for the example-scale models that use Adasum.
+
+Both follow one arithmetic contract for f32 / bf16 / f16 (tests/adasum_oracle.py gives its one correct output and
+tests/test_zzz_adasum_gpu.py holds the kernel to it bit for bit):
+
+* the values are widened to fp32; a.b, |a|^2 and |b|^2 are sums of fp64 products, which are exact for fp32 factors;
+* ``c = fp32(1 - d / (2 n))`` when ``n > 0``, else 1. Nothing is clamped, so the coefficients do not depend on the scale
+  of the tensors: model deltas of norm 1e-20 combine as exactly as gradients of norm 1, and norms past fp32's range
+  (|x| > 2^64) do not overflow;
+* ``z = fp32(fp32(ca a) + fp32(cb b))``; intermediate levels stay fp32, the caller rounds once into the tensor's dtype.
+
+fp64 tensors are combined in fp64 throughout.
 """
 from __future__ import annotations
 
@@ -23,13 +34,17 @@ def _work(t: torch.Tensor) -> torch.Tensor:
     return t if t.dtype == torch.float64 else t.float()     # 16-bit floats are combined in fp32, doubles stay doubles
 
 
+def _coef(dot: torch.Tensor, n: torch.Tensor) -> torch.Tensor:
+    return torch.where(n > 0, 1.0 - dot / (2.0 * n), torch.ones_like(dot))
+
+
 def adasum_pair(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    a32, b32 = _work(a), _work(b)
-    dot = torch.dot(a32.flatten(), b32.flatten())
-    na, nb = a32.pow(2).sum(), b32.pow(2).sum()
-    ca = torch.where(na > 0, 1.0 - dot / (2.0 * na.clamp_min(1e-30)), torch.ones_like(dot))
-    cb = torch.where(nb > 0, 1.0 - dot / (2.0 * nb.clamp_min(1e-30)), torch.ones_like(dot))
-    return ca * a32 + cb * b32
+    a, b = _work(a), _work(b)
+    a64, b64 = a.flatten().double(), b.flatten().double()   # fp64 products of fp32 values are exact
+    dot = torch.dot(a64, b64)
+    na, nb = torch.dot(a64, a64), torch.dot(b64, b64)
+    ca, cb = _coef(dot, na).to(a.dtype), _coef(dot, nb).to(a.dtype)
+    return ca * a + cb * b       # two products and one add, each rounded to the working dtype (no fused multiply-add)
 
 
 def adasum_tree(tensors: List[torch.Tensor]) -> torch.Tensor:

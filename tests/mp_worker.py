@@ -184,17 +184,7 @@ def main():
     torch.cuda.synchronize()
     check("adasum orthogonal", torch.allclose(e, torch.ones_like(e)))
     check("adasum parallel", torch.allclose(p_, torch.full_like(p_, 2.0)))
-
-    # the one-kernel form (csrc/kernels/adasum.cu) on real peers: opt-in until its single-GPU numerics test has passed on hardware
-    if os.environ.get("B200MPI_ADASUM_KERNEL", "0") == "1" and comm.adasum_max_bytes(torch.float32) > 0:
-        from mpi_operator_b200.hvd.adasum import adasum_tree
-        for n in (5, 4099, (1 << 20) + 3):
-            want = adasum_tree([gen(90, n, torch.float32, r) for r in range(W)])
-            got = gen(90, n, torch.float32, R)
-            comm.adasum(got, got)
-            torch.cuda.synchronize()
-            comm.check_error()
-            check(f"adasum kernel n={n}", torch.allclose(got, want, rtol=1e-4, atol=1e-5))
+    # the one-kernel form on real peers, bit for bit: tests/adasum_mp_worker.py (test_zzz_adasum_gpu.py::test_adasum_on_real_peers)
 
     # ---- zero-copy window forms on real peers ----
     per = 1 << 18
