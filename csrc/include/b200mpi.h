@@ -205,6 +205,34 @@ int b200mpi_allreduce_lars_sym(b200mpi_comm_t comm, int grad_win, size_t grad_of
                                const uint16_t* param_map, const uint8_t* param_table, int num_params,
                                int board_win, size_t board_off, void* scratch, size_t scratch_bytes,
                                float eta, void* trust_out);
+/* The grouped SGD step (group_map and group_hyper may both be NULL: the
+ * ungrouped step) and the LARS step, each also keeping an exponential moving
+ * average of the parameters (tf.train.ExponentialMovingAverage with
+ * num_updates). Each launch reads ema_sched = device {d, k} (two doubles: the
+ * decay and the number of parameter updates including this one) and applies
+ *   c  = (float)(1 - min(d, (1 + k) / (10 + k)))     (in double, rounded once)
+ *   e' = fmaf(c, p' - e, e)                           (p' the updated parameter)
+ * to every element of this rank's slice. `ema` is laid out like `momentum`
+ * (b200mpi_slice_elems fp32 elements) and never leaves the rank; the
+ * parameter, momentum, shadow and trust-ratio results are those of the calls
+ * without it. fp32 gradients only; ema and ema_sched must not be NULL.
+ * Emulated mode: `ema` is a host array of world device pointers, ema_sched is
+ * shared. */
+int b200mpi_allreduce_sgd_sym_ema(b200mpi_comm_t comm, int grad_win, size_t grad_off,
+                                  int param_win, size_t param_off, int lowp_win, size_t lowp_off,
+                                  void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale,
+                                  float lr, float mu, float wd, int nesterov, int first_step,
+                                  b200mpi_algo_t algo, void* stream,
+                                  const uint8_t* group_map, const float* group_hyper, int num_groups,
+                                  void* ema, const double* ema_sched);
+int b200mpi_allreduce_lars_sym_ema(b200mpi_comm_t comm, int grad_win, size_t grad_off,
+                                   int param_win, size_t param_off, int lowp_win, size_t lowp_off,
+                                   void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale,
+                                   int nesterov, int first_step, b200mpi_algo_t algo, void* stream,
+                                   const float* group_hyper, int num_groups,
+                                   const uint16_t* param_map, const uint8_t* param_table, int num_params,
+                                   int board_win, size_t board_off, void* scratch, size_t scratch_bytes,
+                                   float eta, void* trust_out, void* ema, const double* ema_sched);
 size_t b200mpi_lars_scratch_bytes(size_t count, int world, int num_params);
 size_t b200mpi_slice_elems(size_t count, int world, b200mpi_dtype_t dtype);
 /* Optional device-resident hyper-parameters {lr, momentum, weight_decay} (3 floats)

@@ -619,13 +619,17 @@ k_allreduce_oneshot(const __grid_constant__ KArgs a0, const KArgs* __restrict__ 
 // {lr, mu, wd} from row a.gmap[i] of the table a.ghyper instead of the
 // kernel-wide values. The flat layout pads every parameter to whole vectors,
 // so a vector never straddles two parameters and one byte per vector is exact.
+// EMA (fp32 gradients only): the owner also folds each updated parameter into
+// its EMA slice a.ema (indexed like the momentum slice, kept only locally) with
+// the coefficient of ema_coef(a.ema_sched).
 // ===========================================================================
-template <typename T, int MODE, bool GROUPS = false>
+template <typename T, int MODE, bool GROUPS = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)
 k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu) {
   EMU_ARGS;
   constexpr int N = VecTraits<T>::N;
   static_assert(!GROUPS || N == 4, "grouped SGD: one map entry per 4-element fp32 vector");
+  static_assert(!EMA || N == 4, "EMA: fp32 gradients only");
   const int rank = a.c.rank, world = a.c.world;
   uint32_t e = a.c.epoch[blockIdx.x];
   const size_t per = a.per, nvec = a.nvec;
@@ -641,6 +645,8 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
   const float lr = a.hyper ? __ldg(a.hyper) : a.lr;
   const float mu = a.hyper ? __ldg(a.hyper + 1) : a.mu;
   const float wd = a.hyper ? __ldg(a.hyper + 2) : a.wd;
+  float ema_c = 0.f;
+  if constexpr (EMA) ema_c = ema_coef(a.ema_sched);  // a.ema_sched aliases dbg: this kernel never reads dbg
 
   // U vectors per thread per trip: U NVLink reduce-loads (or U x world peer loads) are issued before any
   // is consumed — with one vector per trip the NVLS variant was latency-bound.
@@ -694,6 +700,8 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
       float p[N], m[N];
       const float* pl = reinterpret_cast<const float*>(a.param.p[rank]) + el;
       float* ml = a.mom + i * N;
+      float4 ev;  // EMA: this vector of the average, loaded with the parameters (a.ema aliases ustride: never read that here)
+      if constexpr (EMA) ev = *reinterpret_cast<const float4*>(a.ema + i * N);
   #pragma unroll
       for (int q = 0; q < N / 4; q++) {
         float4 t = *reinterpret_cast<const float4*>(pl + 4 * q);
@@ -710,6 +718,9 @@ k_allreduce_sgd(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu)
         m[j] = mj;
         p[j] -= vlr * (a.nesterov ? gj + vmu * mj : mj);
       }
+      if constexpr (EMA)
+        *reinterpret_cast<float4*>(a.ema + i * N) = make_float4(ema_update(ema_c, p[0], ev.x), ema_update(ema_c, p[1], ev.y),
+                                                                ema_update(ema_c, p[2], ev.z), ema_update(ema_c, p[3], ev.w));
   #pragma unroll
       for (int q = 0; q < N / 4; q++) {
         *reinterpret_cast<float4*>(ml + 4 * q) = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
@@ -1117,6 +1128,14 @@ cudaError_t launch_allreduce_sgd(const Launch& l, const KArgs& a, int dtype, int
 cudaError_t launch_allreduce_sgd_groups(const Launch& l, const KArgs& a, int mode) {
   if (mode == MODE_NVLS) return go(k_allreduce_sgd<float, MODE_NVLS, true>, l, a);
   return go(k_allreduce_sgd<float, MODE_P2P, true>, l, a);
+}
+cudaError_t launch_allreduce_sgd_ema(const Launch& l, const KArgs& a, int mode, bool groups) {
+  if (mode == MODE_NVLS) {
+    if (groups) return go(k_allreduce_sgd<float, MODE_NVLS, true, true>, l, a);
+    return go(k_allreduce_sgd<float, MODE_NVLS, false, true>, l, a);
+  }
+  if (groups) return go(k_allreduce_sgd<float, MODE_P2P, true, true>, l, a);
+  return go(k_allreduce_sgd<float, MODE_P2P, false, true>, l, a);
 }
 cudaError_t launch_allgather(const Launch& l, const KArgs& a) { return go(k_allgather, l, a); }
 cudaError_t launch_allgather_sym(const Launch& l, const KArgs& a, int mode) {

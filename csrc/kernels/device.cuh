@@ -316,4 +316,14 @@ __device__ __forceinline__ void user_store(char* base, size_t i, size_t nbytes, 
     if (off + k < nbytes) reinterpret_cast<unsigned char*>(base)[off + k] = b[k];
 }
 
+// Weight average of the fused SGD / LARS steps (tf.train.ExponentialMovingAverage with num_updates): `sched` = device
+// {d, k}, k the number of parameter updates including this one. c_k = fp32(1 - min(d, (1 + k) / (10 + k))), in float64
+// and rounded once, so a host oracle reproduces it exactly; the update is e' = e + c_k * (p' - e) with one rounding per
+// operation (ema_update).
+__device__ __forceinline__ float ema_coef(const double* sched) {
+  const double d = __ldg(sched), k = __ldg(sched + 1);
+  return __double2float_rn(__dsub_rn(1.0, fmin(d, __ddiv_rn(__dadd_rn(1.0, k), __dadd_rn(10.0, k)))));
+}
+__device__ __forceinline__ float ema_update(float c, float p, float e) { return __fmaf_rn(c, __fsub_rn(p, e), e); }
+
 }  // namespace b200mpi

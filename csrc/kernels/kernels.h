@@ -24,7 +24,12 @@ struct KArgs {
   size_t nbytes;    // payload bytes of one logical unit (op specific)
   size_t nvec;      // 16-byte vectors in the logical buffer
   size_t per;       // vectors per rank slice / slot
-  size_t ustride;   // byte stride between per-rank blocks in the user buffer
+  // The weight average of the fused SGD / LARS steps shares this slot and `dbg` with fields those kernels never read:
+  // appending them would grow KArgs, which moves the `emu` parameter and the emulated-args stride of every kernel.
+  union {
+    size_t ustride;   // byte stride between per-rank blocks in the user buffer
+    float* ema;       // fused SGD / LARS with EMA: this rank's EMA slice, indexed like `mom`
+  };
   float scale;
   int op;
   int root;
@@ -41,7 +46,10 @@ struct KArgs {
   // pipelined staged allreduce: lanes x {copy-in, reduce, copy-out} CTAs, `depth` staging slots of `per` vectors per lane
   int lanes;
   int depth;
-  unsigned long long* dbg;   // optional timeline: [role 3][lane kPipeLanes][chunk kPipeDbgChunks][3] globaltimer ns
+  union {
+    unsigned long long* dbg;   // optional timeline: [role 3][lane kPipeLanes][chunk kPipeDbgChunks][3] globaltimer ns
+    const double* ema_sched;   // fused SGD / LARS with EMA: device {decay, updates so far} (ema_coef)
+  };
 };
 constexpr int kPipeDbgChunks = 32;
 
@@ -92,6 +100,8 @@ cudaError_t launch_allreduce_oneshot(const Launch& l, const KArgs& a, int dtype)
 cudaError_t launch_allreduce_sgd(const Launch& l, const KArgs& a, int dtype, int mode);
 // per-vector hyper-parameters from a.gmap / a.ghyper; fp32 gradients only
 cudaError_t launch_allreduce_sgd_groups(const Launch& l, const KArgs& a, int mode);
+// fp32 gradients, grouped or not (a.gmap), plus the weight average in a.ema / a.ema_sched
+cudaError_t launch_allreduce_sgd_ema(const Launch& l, const KArgs& a, int mode, bool groups);
 cudaError_t launch_allgather(const Launch& l, const KArgs& a);
 cudaError_t launch_allgather_sym(const Launch& l, const KArgs& a, int mode);
 cudaError_t launch_broadcast_sym(const Launch& l, const KArgs& a, int mode);
@@ -122,7 +132,7 @@ struct LarsArgs {
 };
 size_t lars_scratch_bytes(size_t per, int P);
 cudaError_t launch_lars_norms(const Launch& l, const KArgs& a, const LarsArgs& L, int mode);
-cudaError_t launch_lars_update(const Launch& l, const KArgs& a, const LarsArgs& L, int mode);
+cudaError_t launch_lars_update(const Launch& l, const KArgs& a, const LarsArgs& L, int mode, bool ema = false);
 cudaError_t launch_scale_cast(cudaStream_t s, const void* in, int in_dt, void* out, int out_dt,
                               size_t count, float scale);
 cudaError_t launch_fill_u32(cudaStream_t s, uint32_t* p, uint32_t v, size_t n);

@@ -162,7 +162,8 @@ k_allreduce_lars_norms(const __grid_constant__ KArgs a0, const KArgs* __restrict
   if (threadIdx.x == 0) a.c.epoch[blockIdx.x] = e;
 }
 
-template <int MODE>
+// EMA: as k_allreduce_sgd's, the owner folds the updated parameters into its EMA slice a.ema.
+template <int MODE, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)
 k_lars_update(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu, const __grid_constant__ LarsArgs L) {
   EMU_ARGS;
@@ -199,6 +200,8 @@ k_lars_update(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu, c
   const size_t base = (size_t)rank * per;
   const size_t lim = base < nvec ? (nvec - base < per ? nvec - base : per) : 0;
   const bool has_lowp = a.lowp.p[0] != nullptr;
+  float ema_c = 0.f;
+  if constexpr (EMA) ema_c = ema_coef(a.ema_sched);  // a.ema_sched aliases dbg: this kernel never reads dbg
   constexpr int U = (MODE == MODE_NVLS) ? 4 : 2;
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x * U + threadIdx.x; i0 < lim; i0 += lars_gstride() * U) {
     int pid[U];
@@ -225,6 +228,8 @@ k_lars_update(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu, c
       const float4 pt = *reinterpret_cast<const float4*>(pl);
       float4 mt = make_float4(0.f, 0.f, 0.f, 0.f);
       if (!a.first_step) mt = *reinterpret_cast<const float4*>(ml);
+      float4 ev;  // EMA: this vector of the average, loaded with the parameters (a.ema aliases ustride: never read that here)
+      if constexpr (EMA) ev = *reinterpret_cast<const float4*>(a.ema + i * 4);
       const float g[4] = {gv[u].x, gv[u].y, gv[u].z, gv[u].w};
       float p[4] = {pt.x, pt.y, pt.z, pt.w};
       float m[4] = {mt.x, mt.y, mt.z, mt.w};
@@ -236,6 +241,9 @@ k_lars_update(const __grid_constant__ KArgs a0, const KArgs* __restrict__ emu, c
         m[j] = mj;
         p[j] = __fmaf_rn(-vlr, a.nesterov ? __fmaf_rn(vmu, mj, dj) : mj, p[j]);
       }
+      if constexpr (EMA)
+        *reinterpret_cast<float4*>(a.ema + i * 4) = make_float4(ema_update(ema_c, p[0], ev.x), ema_update(ema_c, p[1], ev.y),
+                                                                ema_update(ema_c, p[2], ev.z), ema_update(ema_c, p[3], ev.w));
       *reinterpret_cast<float4*>(ml) = make_float4(m[0], m[1], m[2], m[3]);
       const uint4 o = make_uint4(__float_as_uint(p[0]), __float_as_uint(p[1]), __float_as_uint(p[2]), __float_as_uint(p[3]));
       const size_t boff = el * 4;
@@ -275,7 +283,11 @@ cudaError_t launch_lars_norms(const Launch& l, const KArgs& a, const LarsArgs& L
   if (mode == MODE_NVLS) return go_lars(k_allreduce_lars_norms<MODE_NVLS>, l, a, L, smem);
   return go_lars(k_allreduce_lars_norms<MODE_P2P>, l, a, L, smem);
 }
-cudaError_t launch_lars_update(const Launch& l, const KArgs& a, const LarsArgs& L, int mode) {
+cudaError_t launch_lars_update(const Launch& l, const KArgs& a, const LarsArgs& L, int mode, bool ema) {
+  if (ema) {
+    if (mode == MODE_NVLS) return go_lars(k_lars_update<MODE_NVLS, true>, l, a, L, 0);
+    return go_lars(k_lars_update<MODE_P2P, true>, l, a, L, 0);
+  }
   if (mode == MODE_NVLS) return go_lars(k_lars_update<MODE_NVLS>, l, a, L, 0);
   return go_lars(k_lars_update<MODE_P2P>, l, a, L, 0);
 }

@@ -1132,10 +1132,11 @@ int b200mpi_allreduce_sgd_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin,
                                           nesterov, first_step, algo, stream, nullptr, nullptr, 0);
 }
 
-int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
-                                     void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, float lr, float mu,
-                                     float wd, int nesterov, int first_step, b200mpi_algo_t algo, void* stream,
-                                     const uint8_t* group_map, const float* group_hyper, int num_groups) {
+// The fused SGD step behind b200mpi_allreduce_sgd_sym_groups (ema == nullptr) and b200mpi_allreduce_sgd_sym_ema.
+static int sgd_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff, void* momentum,
+                   size_t count, b200mpi_dtype_t gdtype, float scale, float lr, float mu, float wd, int nesterov,
+                   int first_step, b200mpi_algo_t algo, void* stream, const uint8_t* group_map, const float* group_hyper,
+                   int num_groups, void* ema, const double* ema_sched) {
   const bool groups = group_map != nullptr;
   if (groups != (group_hyper != nullptr)) return fail(B200MPI_ERR_INVALID, "allreduce_sgd: group map and group table must be given together");
   if (groups && (num_groups < 1 || num_groups > 256)) return fail(B200MPI_ERR_INVALID, "allreduce_sgd: num_groups must be in [1, 256]");
@@ -1167,11 +1168,39 @@ int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t c, int gwin, size_t goff, in
     a.hyper = c->hyper;
     a.gmap = group_map;      // emulated ranks share one read-only map and table
     a.ghyper = group_hyper;
+    if (ema) {
+      a.ema = reinterpret_cast<float*>(c->local ? reinterpret_cast<void* const*>(ema)[r] : ema);
+      a.ema_sched = ema_sched;
+    }
   }
   return run(c, (cudaStream_t)stream, blocks, "allreduce_sgd", count * esize(gdtype), mode == MODE_NVLS ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT, args,
              [&](const Launch& l, const KArgs& a) {
+               if (ema) return launch_allreduce_sgd_ema(l, a, mode, groups);
                return groups ? launch_allreduce_sgd_groups(l, a, mode) : launch_allreduce_sgd(l, a, gdtype, mode);
              });
+}
+
+int b200mpi_allreduce_sgd_sym_groups(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
+                                     void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, float lr, float mu,
+                                     float wd, int nesterov, int first_step, b200mpi_algo_t algo, void* stream,
+                                     const uint8_t* group_map, const float* group_hyper, int num_groups) {
+  return sgd_sym(c, gwin, goff, pwin, poff, lwin, loff, momentum, count, gdtype, scale, lr, mu, wd, nesterov, first_step, algo,
+                 stream, group_map, group_hyper, num_groups, nullptr, nullptr);
+}
+
+int b200mpi_allreduce_sgd_sym_ema(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
+                                  void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, float lr, float mu,
+                                  float wd, int nesterov, int first_step, b200mpi_algo_t algo, void* stream,
+                                  const uint8_t* group_map, const float* group_hyper, int num_groups, void* ema,
+                                  const double* ema_sched) {
+  if (!ema || !ema_sched) return fail(B200MPI_ERR_INVALID, "allreduce_sgd_ema: ema and ema_sched are required");
+  if (gdtype != B200MPI_F32) return fail(B200MPI_ERR_INVALID, "allreduce_sgd_ema: the weight average needs fp32 gradients");
+  if (c->local) {
+    for (int r = 0; r < c->world; r++)
+      if (!reinterpret_cast<void* const*>(ema)[r]) return fail(B200MPI_ERR_INVALID, "allreduce_sgd_ema: ema needs a pointer per rank");
+  }
+  return sgd_sym(c, gwin, goff, pwin, poff, lwin, loff, momentum, count, gdtype, scale, lr, mu, wd, nesterov, first_step, algo,
+                 stream, group_map, group_hyper, num_groups, ema, ema_sched);
 }
 
 size_t b200mpi_lars_scratch_bytes(size_t count, int world, int num_params) {
@@ -1179,11 +1208,12 @@ size_t b200mpi_lars_scratch_bytes(size_t count, int world, int num_params) {
   return lars_scratch_bytes((nvec + world - 1) / world, num_params);
 }
 
-int b200mpi_allreduce_lars_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
-                               void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, int nesterov,
-                               int first_step, b200mpi_algo_t algo, void* stream, const float* group_hyper, int num_groups,
-                               const uint16_t* param_map, const uint8_t* param_table, int num_params, int bwin,
-                               size_t boff, void* scratch, size_t scratch_bytes, float eta, void* trust_out) {
+// The fused LARS step behind b200mpi_allreduce_lars_sym (ema == nullptr) and b200mpi_allreduce_lars_sym_ema.
+static int lars_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff, void* momentum,
+                    size_t count, b200mpi_dtype_t gdtype, float scale, int nesterov, int first_step, b200mpi_algo_t algo,
+                    void* stream, const float* group_hyper, int num_groups, const uint16_t* param_map,
+                    const uint8_t* param_table, int num_params, int bwin, size_t boff, void* scratch, size_t scratch_bytes,
+                    float eta, void* trust_out, void* ema, const double* ema_sched) {
   if (gdtype != B200MPI_F32) return fail(B200MPI_ERR_INVALID, "allreduce_lars: LARS needs fp32 gradients");
   if (!group_hyper || num_groups < 1 || num_groups > 256) return fail(B200MPI_ERR_INVALID, "allreduce_lars: a group table of 1 to 256 rows is required");
   if (!param_map || !param_table) return fail(B200MPI_ERR_INVALID, "allreduce_lars: parameter map and parameter table must be given together");
@@ -1225,13 +1255,44 @@ int b200mpi_allreduce_lars_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin
     L.scratch[r] = reinterpret_cast<char*>(c->local ? reinterpret_cast<void* const*>(scratch)[r] : scratch);
     if (trust_out) L.trust_out[r] = reinterpret_cast<float*>(c->local ? reinterpret_cast<void* const*>(trust_out)[r] : trust_out);
     if (!L.scratch[r] || ((uintptr_t)L.scratch[r] & 15)) return fail(B200MPI_ERR_INVALID, "allreduce_lars: scratch must be 16-byte aligned");
+    if (ema) {
+      a.ema = reinterpret_cast<float*>(c->local ? reinterpret_cast<void* const*>(ema)[r] : ema);
+      a.ema_sched = ema_sched;
+    }
   }
   const int algo_used = mode == MODE_NVLS ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT;
   int rc = run(c, (cudaStream_t)stream, blocks, "allreduce_lars", count * 4, algo_used, args,
                [&](const Launch& l, const KArgs& a) { return launch_lars_norms(l, a, L, mode); });
   if (rc) return rc;
   return run(c, (cudaStream_t)stream, blocks, "lars_update", 0, algo_used, args,
-             [&](const Launch& l, const KArgs& a) { return launch_lars_update(l, a, L, mode); });
+             [&](const Launch& l, const KArgs& a) { return launch_lars_update(l, a, L, mode, ema != nullptr); });
+}
+
+int b200mpi_allreduce_lars_sym(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
+                               void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, int nesterov,
+                               int first_step, b200mpi_algo_t algo, void* stream, const float* group_hyper, int num_groups,
+                               const uint16_t* param_map, const uint8_t* param_table, int num_params, int bwin,
+                               size_t boff, void* scratch, size_t scratch_bytes, float eta, void* trust_out) {
+  return lars_sym(c, gwin, goff, pwin, poff, lwin, loff, momentum, count, gdtype, scale, nesterov, first_step, algo, stream,
+                  group_hyper, num_groups, param_map, param_table, num_params, bwin, boff, scratch, scratch_bytes, eta,
+                  trust_out, nullptr, nullptr);
+}
+
+int b200mpi_allreduce_lars_sym_ema(b200mpi_comm_t c, int gwin, size_t goff, int pwin, size_t poff, int lwin, size_t loff,
+                                   void* momentum, size_t count, b200mpi_dtype_t gdtype, float scale, int nesterov,
+                                   int first_step, b200mpi_algo_t algo, void* stream, const float* group_hyper,
+                                   int num_groups, const uint16_t* param_map, const uint8_t* param_table, int num_params,
+                                   int bwin, size_t boff, void* scratch, size_t scratch_bytes, float eta, void* trust_out,
+                                   void* ema, const double* ema_sched) {
+  if (!ema || !ema_sched) return fail(B200MPI_ERR_INVALID, "allreduce_lars_ema: ema and ema_sched are required");
+  if (gdtype != B200MPI_F32) return fail(B200MPI_ERR_INVALID, "allreduce_lars_ema: the weight average needs fp32 gradients");
+  if (c->local) {
+    for (int r = 0; r < c->world; r++)
+      if (!reinterpret_cast<void* const*>(ema)[r]) return fail(B200MPI_ERR_INVALID, "allreduce_lars_ema: ema needs a pointer per rank");
+  }
+  return lars_sym(c, gwin, goff, pwin, poff, lwin, loff, momentum, count, gdtype, scale, nesterov, first_step, algo, stream,
+                  group_hyper, num_groups, param_map, param_table, num_params, bwin, boff, scratch, scratch_bytes, eta,
+                  trust_out, ema, ema_sched);
 }
 
 int b200mpi_set_hyper_ptr(b200mpi_comm_t c, const float* p) { c->hyper = p; return 0; }

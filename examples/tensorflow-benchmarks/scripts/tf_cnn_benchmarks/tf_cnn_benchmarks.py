@@ -11,6 +11,7 @@ the reference's sample output (README.md:180-212): a line every 10 steps and a
 final ``total images/sec``.
 """
 import argparse
+import contextlib
 import os
 import sys
 import time
@@ -40,6 +41,9 @@ def main():
     ap.add_argument("--eval", default="False", help="tf_cnn_benchmarks flag: evaluate (forward only) instead of training; restores --train_dir")
     ap.add_argument("--train_dir", default="", help="checkpoint directory (tf_cnn_benchmarks flag): restored from at start if it holds a "
                                                     "checkpoint, written by rank 0 at the end")
+    ap.add_argument("--moving_average_decay", type=float, default=0.0,
+                    help="tf_cnn_benchmarks flag: keep an exponential moving average of the weights with this decay (0: off); "
+                         "--eval evaluates the averaged weights")
     ap.add_argument("--b200_engine", default=os.environ.get("B200MPI_ENGINE", "fused"), choices=["fused", "hvd", "nccl"],
                     help="fused: symmetric-window grads + fused allreduce+SGD kernel in a CUDA graph; "
                          "hvd: hvd.DistributedOptimizer API path; nccl: stock NCCL baseline")
@@ -60,8 +64,12 @@ def main():
     if on_gpu and not torch.cuda.is_available():
         raise SystemExit("tf_cnn_benchmarks (b200): --device=gpu but no CUDA device is visible (use --device=cpu for a host run)")
     evaluating = str(args.eval).lower() == "true"
-    if not on_gpu:   # host run: the Horovod-API engine, except for --eval, which needs the trainer (then with the unfused optimizer)
-        args.b200_engine, args.b200_compute_dtype = ("fused" if evaluating else "hvd"), "fp32"
+    averaging = args.moving_average_decay != 0.0
+    if not on_gpu:   # host run: the Horovod-API engine, except for --eval and the weight average, which need the trainer (then
+        # with the unfused optimizer)
+        args.b200_engine, args.b200_compute_dtype = ("fused" if (evaluating or averaging) else "hvd"), "fp32"
+    if averaging and args.b200_engine not in ("fused", "nccl"):
+        raise SystemExit("tf_cnn_benchmarks (b200): --moving_average_decay needs the trainer engines (fused | nccl)")
     S = args.image_size
     torch.backends.cudnn.benchmark = True
     torch.manual_seed(1234 + rank)
@@ -101,7 +109,8 @@ def main():
             dist.init_process_group("nccl", rank=rank, world_size=size, device_id=torch.device("cuda", torch.cuda.current_device()))
         trainer = DataParallelTrainer(model, loss_fn, hvd._comm(), lr=lr, momentum=mu, weight_decay=args.weight_decay,
                                       autocast_dtype=dtype, comm_backend="nccl" if args.b200_engine == "nccl" else "b200mpi",
-                                      fused_optimizer=on_gpu, cuda_graph=on_gpu)
+                                      fused_optimizer=on_gpu, cuda_graph=on_gpu,
+                                      ema_decay=args.moving_average_decay if averaging else None)
 
         def step():
             return trainer.step(x, y)
@@ -170,13 +179,15 @@ def main():
         # forward-only pass over num_batches synthetic batches: tf_cnn_benchmarks' "Accuracy @ 1 = ... Accuracy @ 5 = ... [N examples]"
         if args.b200_engine not in ("fused", "nccl"):
             raise SystemExit("tf_cnn_benchmarks (b200): --eval needs the trainer engines (fused | nccl)")
+        # with --moving_average_decay under the averaged weights, as tf_cnn_benchmarks' eval restores the averaged variables
         tot = {"top1": 0.0, "top5": 0.0, "n": 0}
         t_ev = time.perf_counter()
-        for _ in range(args.num_batches):
-            r = trainer.evaluate(x, y)
-            tot["top1"] += r.get("top1", 0.0)
-            tot["top5"] += r.get("top5", 0.0)
-            tot["n"] += r["examples"]
+        with (trainer.ema_weights() if averaging else contextlib.nullcontext()):
+            for _ in range(args.num_batches):
+                r = trainer.evaluate(x, y)
+                tot["top1"] += r.get("top1", 0.0)
+                tot["top5"] += r.get("top5", 0.0)
+                tot["n"] += r["examples"]
         device_sync()
         if rank == 0:
             print(f"Accuracy @ 1 = {tot['top1'] / args.num_batches:.4f} Accuracy @ 5 = {tot['top5'] / args.num_batches:.4f} [{tot['n']} examples]")

@@ -21,6 +21,7 @@ GPU-first redesign:
 """
 from __future__ import annotations
 
+import contextlib
 import os
 from dataclasses import dataclass, field
 from typing import Callable, List, Optional
@@ -89,6 +90,7 @@ class Bucket:
     lars: bool = False                       # holds a LARS parameter: runs the fused LARS kernels
     param_table: Optional[torch.Tensor] = None   # [len(params), 2] uint8 {group, lars}, bucket-local parameter order
     trust: Optional[torch.Tensor] = None     # LARS buckets: trust ratio of each parameter at the last synchronising step
+    ema: Optional[torch.Tensor] = None       # ema_decay: this rank's shard of the weight average, sharded like momentum
 
 
 class FlatModelState:
@@ -293,6 +295,19 @@ class DataParallelTrainer:
     else m)``; other parameters keep the plain update (``trust = 1``). ``eta`` is ``trust_coefficient``, trainer-wide and
     fixed at construction. Apex's ``LARC(clip=False)`` differs only where a norm is 0: it then also drops the weight decay.
     ``lars_trust_ratios()`` returns the trust ratios of the last synchronising step.
+
+    ``ema_decay=d`` (``0 < d < 1``) keeps an exponential moving average of the fp32 master of every trainable parameter, as
+    tf_cnn_benchmarks' ``--moving_average_decay`` does with ``tf.train.ExponentialMovingAverage(d, num_updates=step)``. It
+    starts at the broadcast parameters; the k-th synchronising step (k = 1, 2, ..., every step that updated the parameters,
+    the CUDA-graph capture's warm-up steps included) applies ``e = e + c_k * (p - e)`` to the updated parameters ``p`` with
+    ``c_k = 1 - min(d, (1 + k) / (10 + k))``. The fused kernels do it in the same pass as the update, on the slice each rank
+    owns. BatchNorm running statistics are not averaged: they already are averages, and an evaluation under the averaged
+    weights uses the live ones::
+
+        trainer = DataParallelTrainer(model, loss_fn, comm, lr=0.1, ema_decay=0.9999)
+        ...
+        with trainer.ema_weights():            # collective when world > 1
+            print(trainer.evaluate(x, y))
     """
 
     def __init__(self, model: nn.Module, loss_fn: Callable, comm: Communicator, *, lr: float, momentum: float = 0.9,
@@ -300,7 +315,11 @@ class DataParallelTrainer:
                  autocast_dtype: Optional[torch.dtype] = torch.bfloat16, channels_last: bool = True,
                  cuda_graph: bool = True, fused_optimizer: bool = True, algo: Optional[str] = None,
                  comm_backend: str = "b200mpi", bf16_params: Optional[bool] = None, async_h2d: Optional[bool] = None,
-                 param_groups: Optional[list] = None, lars: bool = False, trust_coefficient: float = 0.001):
+                 param_groups: Optional[list] = None, lars: bool = False, trust_coefficient: float = 0.001,
+                 ema_decay: Optional[float] = None):
+        if ema_decay is not None and not (isinstance(ema_decay, (int, float)) and not isinstance(ema_decay, bool)
+                                          and 0.0 < float(ema_decay) < 1.0):
+            raise ValueError(f"ema_decay must be None or a number in (0, 1), got {ema_decay!r}")
         if not isinstance(lars, bool):
             raise ValueError(f"lars must be a bool, got {lars!r}")
         if not (isinstance(trust_coefficient, (int, float)) and float(trust_coefficient) > 0
@@ -352,6 +371,18 @@ class DataParallelTrainer:
         self._lars_board = self._lars_scratch = None
         if self._lars:
             self._alloc_lars()
+        # weight average: {d as fp32 widened, updates so far} on the device, read by the fused kernels (graph replays follow
+        # it); the fused path keeps one shard per bucket beside the momentum, the unfused paths one full flat copy
+        self.ema_decay = None if ema_decay is None else float(torch.tensor(float(ema_decay), dtype=torch.float32))
+        self._ema_sched = None
+        self._flat_ema = None
+        self._in_ema = False
+        if self.ema_decay is not None:
+            self._ema_sched = torch.tensor([self.ema_decay, 0.0], dtype=torch.float64, device=self.device)
+            if self.fused:
+                for b in self.state.buckets:
+                    b.ema = torch.zeros_like(b.momentum)
+            self._set_ema(self.state.flat_param)
         self.comm_stream = torch.cuda.Stream(device=self.device, priority=-1) if self._cuda else None
         self._graph: Optional[torch.cuda.CUDAGraph] = None
         self._static_x = self._static_y = None
@@ -499,6 +530,7 @@ class DataParallelTrainer:
 
     def _reduce_bucket_body(self, b: Bucket) -> None:
         st = self.state
+        ema = {"ema": b.ema, "ema_sched": self._ema_sched} if b.ema is not None else {}
         if self.backend == "nccl":
             g = st.flat_grad[b.start:b.start + b.numel]
             if self.comm.world > 1:
@@ -510,20 +542,20 @@ class DataParallelTrainer:
                                             board_win=self._lars_board, board_off=0, scratch=self._lars_scratch,
                                             trust_coefficient=self.trust_coefficient, nesterov=self.nesterov,
                                             lowp_win=st.lowp_win, lowp_off=b.start * 2, algo=self.algo,
-                                            stream=self.comm_stream, trust_out=b.trust)
+                                            stream=self.comm_stream, trust_out=b.trust, **ema)
         elif self.fused and self._has_groups:
             self.comm.allreduce_sgd_window(st.grad_win, b.start * 4, st.param_win, b.start * 4, b.momentum,
                                            b.numel, torch.float32, lr=self._lr, momentum_coef=self._mu,
                                            weight_decay=self._wd, nesterov=self.nesterov,
                                            lowp_win=st.lowp_win, lowp_off=b.start * 2, algo=self.algo,
                                            stream=self.comm_stream, group_map=st.bucket_group_map(b),
-                                           group_hyper=self.group_hyper)
+                                           group_hyper=self.group_hyper, **ema)
         elif self.fused:
             self.comm.allreduce_sgd_window(st.grad_win, b.start * 4, st.param_win, b.start * 4, b.momentum,
                                            b.numel, torch.float32, lr=self._lr, momentum_coef=self._mu,
                                            weight_decay=self._wd, nesterov=self.nesterov,
                                            lowp_win=st.lowp_win, lowp_off=b.start * 2, algo=self.algo,
-                                           stream=self.comm_stream)
+                                           stream=self.comm_stream, **ema)
         else:
             self.comm.allreduce_window(st.grad_win, b.start * 4, b.numel, torch.float32, op="avg",
                                        algo=self.algo, stream=self.comm_stream)
@@ -554,6 +586,13 @@ class DataParallelTrainer:
         upd = g.add(self._flat_mom, alpha=self._mu) if self.nesterov else self._flat_mom
         st.flat_param.sub_(upd * self.hyper[0])
         st.refresh_lowp()
+
+    def _unfused_ema(self) -> None:
+        """The fused kernels' weight average on the full flat buffers (NCCL baseline and fused_optimizer=False); within 1 ulp
+        of the fused result, which rounds the product and the sum once."""
+        d, k = self._ema_sched[0], self._ema_sched[1]
+        c = (1.0 - torch.minimum(d, (1.0 + k) / (10.0 + k))).float()
+        self._flat_ema.addcmul_(self.state.flat_param - self._flat_ema, c)
 
     def _unfused_trust(self) -> torch.Tensor:
         """LARS trust ratio of every 4-element vector of the flat buffers ([total / 4, 1]; 1 outside LARS parameters), from
@@ -607,6 +646,8 @@ class DataParallelTrainer:
                 loss = self.loss_fn(self.model(x), y)
         if counters:   # one multi-tensor add instead of one tiny kernel per BN layer
             torch._foreach_add_(counters, 1)
+        if self._sync and self._ema_sched is not None:   # k of this update; the bucket kernels read it after the main->comm event
+            self._ema_sched[1:].add_(1)
         with nvtx.range("b200mpi.backward+allreduce_sgd"):   # bucket kernels are launched from the autograd hooks inside
             loss.backward()
         self._loss.copy_(loss.detach())
@@ -620,6 +661,8 @@ class DataParallelTrainer:
             torch.cuda.current_stream(self.device).wait_stream(self.comm_stream)
         if not self.fused:
             self._unfused_sgd()
+            if self._flat_ema is not None:
+                self._unfused_ema()
         self._carry = False
 
     def _ensure_static(self, x, y):
@@ -684,6 +727,8 @@ class DataParallelTrainer:
     def step(self, x=None, y=None):
         """One optimizer step on a batch given as (pinned) host or device tensors; without arguments, on the batch handed
         to ``prefetch()``. Returns the loss as a device scalar (``float(loss)`` is the D2H read)."""
+        if self._in_ema:
+            raise RuntimeError("step() inside ema_weights(): the parameter window holds the averaged weights")
         self._fault.on_step()
         if x is not None:
             self.prefetch(x, y)
@@ -815,22 +860,15 @@ class DataParallelTrainer:
         world > 1: the fused optimizer keeps only 1/world of every bucket's momentum on each rank, so the shards are
         all-gathered first (one byte-wise allgather kernel per bucket); every rank gets the full dictionary, write it from rank 0.
         Loading re-shards for whatever world the new trainer runs in (elastic rescale, different GPU count)."""
+        if self._in_ema:
+            raise RuntimeError("state_dict() inside ema_weights(): the parameter window holds the averaged weights")
         st = self.state
         names = {p: n for n, p in self.model.named_parameters()}
         if self._cuda:
             torch.cuda.synchronize(self.device)
         mom_flat = torch.zeros(st.total, dtype=torch.float32, device=st.flat_param.device)
         if self.fused:
-            W = self.comm.world
-            for b in st.buckets:
-                per = b.momentum.numel()
-                full = b.momentum
-                if W > 1:
-                    full = torch.empty(W * per, dtype=torch.float32, device=b.momentum.device)
-                    self.comm.allgather(b.momentum, full)
-                mom_flat[b.start:b.start + b.numel] = full[:b.numel]
-            if self._cuda:
-                torch.cuda.synchronize(self.device)
+            mom_flat = self._gather_shards("momentum")
         elif hasattr(self, "_flat_mom"):
             mom_flat.copy_(self._flat_mom)
         masters, momentum = {}, {}
@@ -846,7 +884,85 @@ class DataParallelTrainer:
               "world_size_at_save": int(self.comm.world)}
         if self._has_groups:
             sd["param_groups"] = self.param_groups
+        if self.ema_decay is not None:
+            ema_flat = self._gather_ema()
+            sd["ema"] = {names[p]: ema_flat[st.param_slot[p][1]:st.param_slot[p][1] + p.numel()].as_strided(p.size(), p.stride())
+                         .detach().cpu().contiguous() for p in st.params}
+            sd["ema_updates"] = self.ema_updates
+            sd["hyper"]["ema_decay"] = self.ema_decay
         return sd
+
+    def _gather_shards(self, attr: str) -> torch.Tensor:
+        """The full flat fp32 buffer of a per-bucket sharded state (``"momentum"`` or ``"ema"``); one allgather per bucket,
+        COLLECTIVE when world > 1."""
+        st = self.state
+        out = torch.zeros(st.total, dtype=torch.float32, device=st.flat_param.device)
+        W = self.comm.world
+        for b in st.buckets:
+            shard = getattr(b, attr)
+            full = shard
+            if W > 1:
+                full = torch.empty(W * shard.numel(), dtype=torch.float32, device=shard.device)
+                self.comm.allgather(shard, full)
+            out[b.start:b.start + b.numel] = full[:b.numel]
+        if self._cuda:
+            torch.cuda.synchronize(self.device)
+        return out
+
+    def _gather_ema(self) -> torch.Tensor:
+        """The weight average as one full flat fp32 buffer (COLLECTIVE on the fused path when world > 1)."""
+        if self._cuda:
+            torch.cuda.synchronize(self.device)
+        return self._gather_shards("ema") if self.fused else self._flat_ema.clone()
+
+    def _set_ema(self, flat: torch.Tensor) -> None:
+        """Make the weight average ``flat`` (a full flat fp32 buffer): this rank's shard of every bucket, or the flat copy."""
+        st = self.state
+        if not self.fused:
+            # in place once it exists: a captured graph (comm_backend="nccl") keeps updating this buffer
+            if self._flat_ema is None:
+                self._flat_ema = flat.detach().clone()
+            else:
+                self._flat_ema.copy_(flat)
+            return
+        r = self.comm.rank
+        for b in st.buckets:
+            per = b.ema.numel()
+            lo, hi = min(r * per, b.numel), min((r + 1) * per, b.numel)
+            b.ema.zero_()
+            b.ema[:hi - lo] = flat[b.start + lo:b.start + hi]
+
+    @property
+    def ema_updates(self) -> int:
+        """k: the number of parameter updates the weight average has seen (reading it synchronises with the device)."""
+        return int(self._ema_sched[1]) if self._ema_sched is not None else 0
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Context manager: inside it the model's parameters (fp32 masters and the bf16 shadow) hold the weight average, so
+        ``evaluate()`` (its CUDA graphs included) runs on the averaged weights with the live BatchNorm statistics; on exit the
+        trained parameters are restored bit for bit. ``step()`` and ``state_dict()`` inside it raise ``RuntimeError``.
+        COLLECTIVE when world > 1 (the shards are all-gathered on entry)."""
+        if self.ema_decay is None:
+            raise RuntimeError("ema_weights() needs a trainer built with ema_decay")
+        if self._in_ema:
+            raise RuntimeError("ema_weights() is already active")
+        st = self.state
+        ema_flat = self._gather_ema()
+        with torch.no_grad():
+            saved = st.flat_param.clone()
+            st.flat_param.copy_(ema_flat)
+            st.refresh_lowp()
+        self._in_ema = True
+        try:
+            yield self
+        finally:
+            with torch.no_grad():
+                st.flat_param.copy_(saved)
+                st.refresh_lowp()
+            self._in_ema = False
+            if self._cuda:
+                torch.cuda.synchronize(self.device)
 
     def load_state_dict(self, sd: dict, load_hyper: bool = True) -> None:
         """Restore ``state_dict()`` output in a trainer built on the same model class (any world size, with or without the bf16
@@ -854,7 +970,12 @@ class DataParallelTrainer:
         With ``load_hyper``, per-group values are restored when the checkpoint's parameter groups have the same members (by
         name) as this trainer's; a checkpoint with groups into a trainer without them, or the reverse, is a ``ValueError``.
         Which groups use LARS and ``trust_coefficient`` stay as this trainer was built (the checkpoint records them): the
-        momentum is the same state for SGD and LARS, so SGD and LARS checkpoints load into each other."""
+        momentum is the same state for SGD and LARS, so SGD and LARS checkpoints load into each other. With ``ema_decay`` the
+        weight average and its update count are restored from ``"ema"`` / ``"ema_updates"``, or, for a checkpoint without
+        them, restart from the loaded parameters at count 0; the decay stays this trainer's. Without ``ema_decay`` they are
+        ignored."""
+        if self._in_ema:
+            raise RuntimeError("load_state_dict() inside ema_weights(): leaving the context would undo it")
         if sd.get("format") != "b200mpi.DataParallelTrainer/1":
             raise ValueError("not a DataParallelTrainer checkpoint")
         if load_hyper and ("param_groups" in sd) != self._has_groups:
@@ -894,6 +1015,15 @@ class DataParallelTrainer:
                     b.momentum[:hi - lo] = mom_flat[b.start + lo:b.start + hi]
             else:
                 self._flat_mom = mom_flat
+            if self.ema_decay is not None:
+                ema_flat = st.flat_param.clone()
+                for p in st.params:
+                    name = names[p]
+                    if name in sd.get("ema", {}):
+                        start, n = st.param_slot[p][1], p.numel()
+                        ema_flat[start:start + n].as_strided(p.size(), p.stride()).copy_(sd["ema"][name].to(dev, torch.float32))
+                self._set_ema(ema_flat)
+                self._ema_sched[1] = float(sd.get("ema_updates", 0)) if "ema" in sd else 0.0
         if load_hyper and "hyper" in sd:
             h = sd["hyper"]
             self._lr, self._mu, self._wd = h["lr"], h["momentum"], h["weight_decay"]

@@ -82,6 +82,10 @@ def lib() -> C.CDLL:
     L.b200mpi_allreduce_sgd_sym_groups.argtypes = [vp, i, sz, i, sz, i, sz, vp, sz, i, f, f, f, f, i, i, i, vp, vp, vp, i]
     L.b200mpi_allreduce_lars_sym.argtypes = [vp, i, sz, i, sz, i, sz, vp, sz, i, f, i, i, i, vp, vp, i, vp, vp, i, i, sz,
                                              vp, sz, f, vp]
+    L.b200mpi_allreduce_sgd_sym_ema.argtypes = [vp, i, sz, i, sz, i, sz, vp, sz, i, f, f, f, f, i, i, i, vp, vp, vp, i,
+                                                vp, vp]
+    L.b200mpi_allreduce_lars_sym_ema.argtypes = [vp, i, sz, i, sz, i, sz, vp, sz, i, f, i, i, i, vp, vp, i, vp, vp, i, i,
+                                                 sz, vp, sz, f, vp, vp, vp]
     L.b200mpi_lars_scratch_bytes.argtypes = [sz, i, i]
     L.b200mpi_lars_scratch_bytes.restype = sz
     L.b200mpi_slice_elems.argtypes = [sz, i, i]

@@ -329,39 +329,78 @@ class Communicator:
                              count: int, grad_dtype, lr: float, momentum_coef: float = 0.0, weight_decay: float = 0.0,
                              nesterov: bool = False, first_step: bool = False, scale: Optional[float] = None,
                              lowp_win: Optional[Window] = None, lowp_off: int = 0, algo=None, stream=None,
-                             group_map=None, group_hyper=None) -> None:
+                             group_map=None, group_hyper=None, ema=None, ema_sched=None) -> None:
         """Fused gradient-average + SGD step; see b200mpi_allreduce_sgd_sym.
 
         Parameter groups (fp32 gradients only): ``group_map`` is a CUDA uint8 tensor of ``count // 4`` entries, the group of
         each 4-element vector of this region (already offset to it), and ``group_hyper`` a contiguous CUDA float32 ``[G, 3]``
         tensor of ``{lr, momentum, weight_decay}`` rows, read by the kernel at run time, which then replaces ``lr``,
         ``momentum_coef``, ``weight_decay`` and ``set_hyper``'s tensor. Every map entry must be ``< G``; the kernel does not
-        check it. On an emulated communicator one map and one table serve every rank."""
+        check it. On an emulated communicator one map and one table serve every rank.
+
+        Weight average (fp32 gradients only; see b200mpi_allreduce_sgd_sym_ema): ``ema`` is this rank's float32 shard of
+        ``slice_elems(count)`` elements, laid out like ``momentum`` (emulated: a list of ``world``), and ``ema_sched`` a
+        contiguous float64 CUDA tensor ``[decay, updates]`` read at run time; the two go together."""
         pm, _ = self._ptrs(momentum)
         s = (1.0 / self.world) if scale is None else float(scale)
+        pe = self._ema_ptrs("allreduce_sgd_window", count, grad_dtype, ema, ema_sched)
+        if pe is not None:
+            check(_lib.lib().b200mpi_allreduce_sgd_sym_ema(
+                self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm,
+                count, dtype_code(grad_dtype), s, lr, momentum_coef, weight_decay, int(nesterov), int(first_step),
+                resolve_algo(algo), _stream_ptr(stream),
+                *self._group_ptrs("allreduce_sgd_window", count, grad_dtype, group_map, group_hyper), *pe),
+                "allreduce_sgd_sym_ema")
+            return
         if group_map is not None or group_hyper is not None:
-            torch = _torch()
-            if group_map is None or group_hyper is None:
-                raise B200MPIError("allreduce_sgd_window: group_map and group_hyper go together")
-            if grad_dtype != torch.float32:
-                raise B200MPIError("allreduce_sgd_window: parameter groups need float32 gradients")
-            dev = torch.device("cuda", self.device)
-            if not (group_map.device == dev and group_map.dtype == torch.uint8 and group_map.is_contiguous()
-                    and group_map.numel() == count // 4):
-                raise B200MPIError(f"allreduce_sgd_window: group_map must be a contiguous uint8 tensor of {count // 4} entries on {dev}")
-            if not (group_hyper.device == dev and group_hyper.dtype == torch.float32 and group_hyper.is_contiguous()
-                    and group_hyper.dim() == 2 and group_hyper.shape[1] == 3 and 1 <= group_hyper.shape[0] <= 256):
-                raise B200MPIError(f"allreduce_sgd_window: group_hyper must be a contiguous float32 [G, 3] tensor on {dev}, 1 <= G <= 256")
             check(_lib.lib().b200mpi_allreduce_sgd_sym_groups(
                 self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm,
                 count, dtype_code(grad_dtype), s, lr, momentum_coef, weight_decay, int(nesterov), int(first_step),
-                resolve_algo(algo), _stream_ptr(stream), group_map.data_ptr(), group_hyper.data_ptr(),
-                int(group_hyper.shape[0])), "allreduce_sgd_sym_groups")
+                resolve_algo(algo), _stream_ptr(stream),
+                *self._group_ptrs("allreduce_sgd_window", count, grad_dtype, group_map, group_hyper)),
+                "allreduce_sgd_sym_groups")
             return
         check(_lib.lib().b200mpi_allreduce_sgd_sym(
             self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm,
             count, dtype_code(grad_dtype), s, lr, momentum_coef, weight_decay, int(nesterov), int(first_step),
             resolve_algo(algo), _stream_ptr(stream)), "allreduce_sgd_sym")
+
+    def _group_ptrs(self, name: str, count: int, grad_dtype, group_map, group_hyper) -> tuple:
+        """Checked (map, table, rows) of the grouped entry points: all null without parameter groups."""
+        if group_map is None and group_hyper is None:
+            return None, None, 0
+        torch = _torch()
+        dev = torch.device("cuda", self.device)
+        if group_map is None or group_hyper is None:
+            raise B200MPIError(f"{name}: group_map and group_hyper go together")
+        if grad_dtype != torch.float32:
+            raise B200MPIError(f"{name}: parameter groups need float32 gradients")
+        if not (group_map.device == dev and group_map.dtype == torch.uint8 and group_map.is_contiguous()
+                and group_map.numel() == count // 4):
+            raise B200MPIError(f"{name}: group_map must be a contiguous uint8 tensor of {count // 4} entries on {dev}")
+        if not (group_hyper.device == dev and group_hyper.dtype == torch.float32 and group_hyper.is_contiguous()
+                and group_hyper.dim() == 2 and group_hyper.shape[1] == 3 and 1 <= group_hyper.shape[0] <= 256):
+            raise B200MPIError(f"{name}: group_hyper must be a contiguous float32 [G, 3] tensor on {dev}, 1 <= G <= 256")
+        return group_map.data_ptr(), group_hyper.data_ptr(), int(group_hyper.shape[0])
+
+    def _ema_ptrs(self, name: str, count: int, grad_dtype, ema, ema_sched) -> Optional[tuple]:
+        """Checked (ema, ema_sched) pointers of the ``_ema`` entry points, or None when neither is given."""
+        if ema is None and ema_sched is None:
+            return None
+        torch = _torch()
+        dev = torch.device("cuda", self.device)
+        if ema is None or ema_sched is None:
+            raise B200MPIError(f"{name}: ema and ema_sched go together")
+        if grad_dtype != torch.float32:
+            raise B200MPIError(f"{name}: the weight average needs float32 gradients")
+        n = self.slice_elems(count, torch.float32)
+        shards = ema if isinstance(ema, (list, tuple)) else [ema]
+        if any(not (t.device == dev and t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n) for t in shards):
+            raise B200MPIError(f"{name}: ema must be contiguous float32 tensors of {n} elements on {dev}")
+        if not (ema_sched.device == dev and ema_sched.dtype == torch.float64 and ema_sched.is_contiguous()
+                and ema_sched.numel() == 2):
+            raise B200MPIError(f"{name}: ema_sched must be a contiguous float64 tensor of 2 elements on {dev}")
+        return self._ptrs(ema)[0], ema_sched.data_ptr()
 
     def lars_scratch_bytes(self, count: int, num_params: int) -> int:
         """Bytes of the per-rank scratch ``allreduce_lars_window`` needs for a region of ``count`` fp32 elements."""
@@ -371,7 +410,8 @@ class Communicator:
                               count: int, grad_dtype, *, group_hyper, param_map, param_table, board_win: Window,
                               board_off: int, scratch, trust_coefficient: float, nesterov: bool = False,
                               first_step: bool = False, scale: Optional[float] = None, lowp_win: Optional[Window] = None,
-                              lowp_off: int = 0, algo=None, stream=None, trust_out=None) -> None:
+                              lowp_off: int = 0, algo=None, stream=None, trust_out=None, ema=None,
+                              ema_sched=None) -> None:
         """Fused gradient-average + LARS step; see b200mpi_allreduce_lars_sym. Two launches on ``stream``.
 
         ``param_map`` is a CUDA uint16 tensor of ``count // 4`` entries, the bucket-local parameter of each 4-element vector
@@ -379,7 +419,8 @@ class Communicator:
         tensor of ``{group, lars}`` rows and ``group_hyper`` the ``[G, 3]`` table of ``allreduce_sgd_window``. ``board_win``
         holds ``P * world`` float pairs at ``board_off``. ``scratch`` is this rank's zero-filled CUDA uint8 tensor of at
         least ``lars_scratch_bytes(count, P)`` bytes and ``trust_out`` an optional float32 ``[P]`` tensor that receives the
-        trust ratios (on an emulated communicator: lists of ``world`` tensors, one per rank)."""
+        trust ratios (on an emulated communicator: lists of ``world`` tensors, one per rank). ``ema`` / ``ema_sched`` add the
+        weight average of ``allreduce_sgd_window``."""
         torch = _torch()
         if grad_dtype != torch.float32:
             raise B200MPIError("allreduce_lars_window: LARS needs float32 gradients")
@@ -405,6 +446,15 @@ class Communicator:
         ps, _ = self._ptrs(scratch)
         pt = self._ptrs(trust_out)[0] if trust_out is not None else None
         s = (1.0 / self.world) if scale is None else float(scale)
+        pe = self._ema_ptrs("allreduce_lars_window", count, grad_dtype, ema, ema_sched)
+        if pe is not None:
+            check(_lib.lib().b200mpi_allreduce_lars_sym_ema(
+                self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm,
+                count, dtype_code(grad_dtype), s, int(nesterov), int(first_step), resolve_algo(algo), _stream_ptr(stream),
+                group_hyper.data_ptr(), int(group_hyper.shape[0]), param_map.data_ptr(), param_table.data_ptr(), P,
+                board_win.id, board_off, ps, min(t.numel() for t in scr), float(trust_coefficient), pt, *pe),
+                "allreduce_lars_sym_ema")
+            return
         check(_lib.lib().b200mpi_allreduce_lars_sym(
             self._h, grad_win.id, grad_off, param_win.id, param_off, lowp_win.id if lowp_win else -1, lowp_off, pm, count,
             dtype_code(grad_dtype), s, int(nesterov), int(first_step), resolve_algo(algo), _stream_ptr(stream),
