@@ -622,6 +622,21 @@ k_allreduce_oneshot(const __grid_constant__ KArgs a0, const KArgs* __restrict__ 
 // EMA (fp32 gradients only): the owner also folds each updated parameter into
 // its EMA slice a.ema (indexed like the momentum slice, kept only locally) with
 // the coefficient of ema_coef(a.ema_sched).
+//
+// The update's roundings (tests/optimizer_oracle.py states them on the host):
+//   S  = fp32 sum of the ranks' gradients (widened to fp32) in the slice
+//        owner's order: owner, owner+1, ... (mod world). NVLS: multimem
+//        ld_reduce; bf16 / f16 sums come back rounded to T.
+//   d  = __fmaf_rn(S, scale, __fmul_rn(wd, p))
+//   m' = first_step ? d : __fmaf_rn(mu, m, d)
+//   p' = __fmaf_rn(-lr, nesterov ? __fmaf_rn(mu, m', d) : m', p)
+//   shadow = bf16 round-to-nearest-even of p'
+// The loop below is plain C: nvcc contracts it to exactly these FMAs in every
+// instantiation, and tests/test_fused_optimizer_exact_gpu.py holds each one to
+// them bit for bit. Spelled with the intrinsics, the first_step / nesterov
+// selects became branches or the address code was rescheduled, and the step
+// ran 1-5% slower (H100 80GB HBM3, 700 W power limit).
+// k_lars_update runs the same expressions with d scaled by the trust ratio.
 // ===========================================================================
 template <typename T, int MODE, bool GROUPS = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)

@@ -23,8 +23,20 @@
 //
 // Every sum has a fixed order and there are no float atomics, so all ranks and all runs agree bit for bit. For vectors of
 // non-LARS parameters trust is exactly 1 and the update is written with the FMAs k_allreduce_sgd compiles to, so they come
-// out bitwise equal to the grouped kernel. Extra HBM traffic over k_allreduce_sgd per rank: one read of the parameter
-// slice (norms) and one write + one read of the sum scratch: 3 * S / world for S bytes of fp32 parameters.
+// out bitwise equal to the grouped kernel.
+//
+// The trust contract, in fp32 throughout (tests/optimizer_oracle.py states it on the host), with S the fp32 sum of the
+// ranks' gradients as in k_allreduce_sgd:
+//   gs = fp32(S * scale)
+//   sg, sp = fp32 sums of fmaf(gs, gs, .) / fmaf(w, w, .) over the parameter's elements of each slice, then over ranks
+//            0..world-1 (the order within a slice follows the grid: the host can only bound it)
+//   gn = sqrtf(sg), wn = sqrtf(sp)
+//   t  = (wn > 0 && gn > 0) ? fdiv(fmul(eta, wn), fadd(fmaf(wd, wn, gn), kLarsEps)) : 1
+//   d  = fmul(t, fmaf(S, scale, fmul(wd, p)))
+// so NaN norms give t = 1 and an fp32 overflow of sg (gn = inf) gives t = 0.
+//
+// Extra HBM traffic over k_allreduce_sgd per rank: one read of the parameter slice (norms) and one write + one read of the
+// sum scratch: 3 * S / world for S bytes of fp32 parameters.
 #include "kernels.h"
 
 namespace b200mpi {

@@ -44,10 +44,11 @@ def fma32(a: np.ndarray, b: np.ndarray, c: np.ndarray) -> np.ndarray:
     t = (prod - (s - bb)) + (cc - bb)
     out = s.astype(np.float32)
     # RN32(s) == RN32(s + t) unless s is an fp32 midpoint (a midpoint strictly between s and s + t would be closer to the
-    # exact value than s is) and t != 0; those elements, and any tie, are rounded from the exact value
+    # exact value than s is) and t != 0; those elements are rounded from the exact value (with t == 0, s is exact and the
+    # cast above already rounded a tie to even)
     lo = out.astype(np.float64)
     other = np.where(lo <= s, np.nextafter(out, np.float32(np.inf)), np.nextafter(out, np.float32(-np.inf))).astype(np.float64)
-    mid = (lo + other) * 0.5 == s
+    mid = ((lo + other) * 0.5 == s) & (t != 0)
     for i in zip(*np.nonzero(mid)):
         x = Fraction(float(a[i])) * Fraction(float(b[i])) + Fraction(float(c[i]))
         out[i] = _round_exact(x, out[i])
