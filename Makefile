@@ -9,7 +9,7 @@ CXXFLAGS  := -std=c++17 -O2 -fPIC -Wall -Icsrc/include
 LIBDIR    := mpi_operator_b200/lib
 BINDIR    := mpi_operator_b200/bin
 
-RUNTIME_SRCS := csrc/kernels/collectives.cu csrc/kernels/adasum.cu csrc/kernels/lars.cu csrc/kernels/bn_act.cu csrc/kernels/p2p.cu csrc/runtime/comm.cc csrc/runtime/rendezvous.cc
+RUNTIME_SRCS := csrc/kernels/collectives.cu csrc/kernels/adasum.cu csrc/kernels/lars.cu csrc/kernels/lr_schedule.cu csrc/kernels/bn_act.cu csrc/kernels/p2p.cu csrc/runtime/comm.cc csrc/runtime/rendezvous.cc
 RUNTIME_HDRS := csrc/include/b200mpi.h csrc/kernels/device.cuh csrc/kernels/kernels.h csrc/kernels/gemm_bnstats_logic.h csrc/runtime/rendezvous.h
 
 all: $(LIBDIR)/libb200mpi.so $(LIBDIR)/libb200mpi_nccl.so $(LIBDIR)/libb200mpi_gemm.so native

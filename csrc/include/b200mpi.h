@@ -239,6 +239,21 @@ size_t b200mpi_slice_elems(size_t count, int world, b200mpi_dtype_t dtype);
  * read by the fused kernels instead of the by-value arguments: a captured CUDA
  * graph then follows LR schedules without re-capture. NULL restores by-value. */
 int b200mpi_set_hyper_ptr(b200mpi_comm_t comm, const float* device_hyper);
+/* Learning-rate schedule step (one single-CTA launch on `stream`): reads the
+ * device step counter k, evaluates the multiplier m(k) of the float64 device
+ * table `schedule` in float64 and writes
+ *   hyper[0] = fp32_rn(base[0] * m(k)),  group_hyper[3*g] = fp32_rn(base[g] * m(k))  (g < num_groups)
+ * then stores k + 1. The momentum and weight-decay entries are not touched.
+ * `form` (0 constant, 1 piecewise, 2 exponential, 3 polynomial) and
+ * `num_boundaries` (piecewise: 0..64, otherwise 0) say how to decode the table:
+ *   [0] warm-up steps W, then  piecewise: num_boundaries boundaries and
+ *   num_boundaries + 1 multipliers; exponential: decay_steps, factor, floor;
+ *   polynomial: total steps T, power, end.
+ * mpi_operator_b200/parallel/lr_schedule.py states the contract and builds the
+ * table. `base` holds num_groups (1..256) doubles; group_hyper ([num_groups][3]
+ * floats) may be NULL, every other pointer may not. */
+int b200mpi_lr_schedule(b200mpi_comm_t comm, const double* schedule, int form, int num_boundaries, int64_t* step,
+                        const double* base, int num_groups, float* hyper, float* group_hyper, void* stream);
 
 int b200mpi_broadcast(b200mpi_comm_t comm, void* buf, size_t count, b200mpi_dtype_t dtype,
                       int root, void* stream);

@@ -133,6 +133,12 @@ struct LarsArgs {
 size_t lars_scratch_bytes(size_t per, int P);
 cudaError_t launch_lars_norms(const Launch& l, const KArgs& a, const LarsArgs& L, int mode);
 cudaError_t launch_lars_update(const Launch& l, const KArgs& a, const LarsArgs& L, int mode, bool ema = false);
+// Learning-rate schedule (lr_schedule.cu): one CTA; reads the step count, writes each group's rate, stores count + 1.
+enum : int { LR_CONSTANT = 0, LR_PIECEWISE = 1, LR_EXPONENTIAL = 2, LR_POLYNOMIAL = 3 };
+constexpr int kLrMaxBoundaries = 64;
+constexpr int kLrMaxGroups = 256;
+cudaError_t launch_lr_schedule(cudaStream_t s, const double* sched, int form, int nb, long long* step, const double* base,
+                               int G, float* hyper, float* group_hyper);
 cudaError_t launch_scale_cast(cudaStream_t s, const void* in, int in_dt, void* out, int out_dt,
                               size_t count, float scale);
 cudaError_t launch_fill_u32(cudaStream_t s, uint32_t* p, uint32_t v, size_t n);

@@ -1297,6 +1297,20 @@ int b200mpi_allreduce_lars_sym_ema(b200mpi_comm_t c, int gwin, size_t goff, int 
 
 int b200mpi_set_hyper_ptr(b200mpi_comm_t c, const float* p) { c->hyper = p; return 0; }
 
+int b200mpi_lr_schedule(b200mpi_comm_t c, const double* schedule, int form, int num_boundaries, int64_t* step,
+                        const double* base, int num_groups, float* hyper, float* group_hyper, void* stream) {
+  if (!c || !schedule || !step || !base || !hyper) return fail(B200MPI_ERR_INVALID, "lr_schedule: schedule, step, base and hyper are required");
+  if (num_groups < 1 || num_groups > kLrMaxGroups) return fail(B200MPI_ERR_INVALID, "lr_schedule: num_groups must be in [1, 256]");
+  if (form < LR_CONSTANT || form > LR_POLYNOMIAL || num_boundaries < 0 || num_boundaries > kLrMaxBoundaries ||
+      (form != LR_PIECEWISE && num_boundaries != 0))
+    return fail(B200MPI_ERR_INVALID, "lr_schedule: unknown schedule form or boundary count");
+  const cudaError_t e = launch_lr_schedule((cudaStream_t)stream, schedule, form, num_boundaries,
+                                           reinterpret_cast<long long*>(step), base, num_groups, hyper, group_hyper);
+  if (e != cudaSuccess) return fail(B200MPI_ERR_CUDA, std::string("lr_schedule launch: ") + cudaGetErrorString(e));
+  c->launches.fetch_add(1, std::memory_order_relaxed);
+  return 0;
+}
+
 int b200mpi_broadcast_bytes(b200mpi_comm_t c, void* buf, size_t bytes, int root, void* stream) {
   if (root < 0 || root >= c->world) return fail(B200MPI_ERR_INVALID, "broadcast: bad root");
   const int mode = c->multicast ? MODE_NVLS : MODE_P2P;

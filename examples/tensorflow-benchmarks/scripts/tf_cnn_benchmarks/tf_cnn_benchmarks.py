@@ -44,6 +44,17 @@ def main():
     ap.add_argument("--moving_average_decay", type=float, default=0.0,
                     help="tf_cnn_benchmarks flag: keep an exponential moving average of the weights with this decay (0: off); "
                          "--eval evaluates the averaged weights")
+    ap.add_argument("--piecewise_learning_rate_schedule", default="",
+                    help='tf_cnn_benchmarks flag: "v0;e1;v1;e2;v2;..." - learning rate v0 until epoch e1, v1 until e2, ...; '
+                         "takes precedence over --init_learning_rate")
+    ap.add_argument("--num_learning_rate_warmup_epochs", type=float, default=0.0,
+                    help="tf_cnn_benchmarks flag: ramp the learning rate linearly from 0 over this many epochs")
+    ap.add_argument("--num_epochs_per_decay", type=float, default=0.0,
+                    help="tf_cnn_benchmarks flag: with --learning_rate_decay_factor, multiply the learning rate by the factor "
+                         "every this many epochs (staircase)")
+    ap.add_argument("--learning_rate_decay_factor", type=float, default=0.0, help="tf_cnn_benchmarks flag: see --num_epochs_per_decay")
+    ap.add_argument("--minimum_learning_rate", type=float, default=0.0,
+                    help="tf_cnn_benchmarks flag: lower bound of the exponentially decayed learning rate")
     ap.add_argument("--b200_engine", default=os.environ.get("B200MPI_ENGINE", "fused"), choices=["fused", "hvd", "nccl"],
                     help="fused: symmetric-window grads + fused allreduce+SGD kernel in a CUDA graph; "
                          "hvd: hvd.DistributedOptimizer API path; nccl: stock NCCL baseline")
@@ -57,6 +68,7 @@ def main():
     import mpi_operator_b200.hvd as hvd
     from mpi_operator_b200.models import build_model
     from mpi_operator_b200.parallel.data_parallel import DataParallelTrainer
+    from mpi_operator_b200.parallel.lr_schedule import LRSchedule
 
     hvd.init()
     rank, size = hvd.rank(), hvd.size()
@@ -76,6 +88,29 @@ def main():
     mu = args.momentum if args.optimizer == "momentum" or args.momentum else 0.0
     lr = args.init_learning_rate * size  # Horovod convention (tensorflow_mnist.py:123-130)
     B = args.batch_size
+    # learning-rate schedule, tf_cnn_benchmarks' get_learning_rate: epochs count images of the global batch, every rate is
+    # scaled by the world size like --init_learning_rate, and the warm-up ramps to the first rate
+    steps_per_epoch = 1281167.0 / (B * size)
+    warmup = int(steps_per_epoch * args.num_learning_rate_warmup_epochs) if args.num_learning_rate_warmup_epochs > 0 else 0
+    lr_schedule = None
+    try:
+        if args.piecewise_learning_rate_schedule:
+            parts = args.piecewise_learning_rate_schedule.split(";")
+            vals, epochs = [float(v) for v in parts[0::2]], [float(e) for e in parts[1::2]]
+            if len(parts) % 2 != 1 or not vals[0] > 0:
+                raise ValueError("--piecewise_learning_rate_schedule needs 'v0;e1;v1;...' with v0 > 0")
+            lr = vals[0] * size
+            lr_schedule = LRSchedule.piecewise([int(steps_per_epoch * e) for e in epochs], [v / vals[0] for v in vals],
+                                               warmup_steps=warmup)
+        elif args.num_epochs_per_decay > 0 and args.learning_rate_decay_factor > 0:
+            if not args.init_learning_rate > 0:
+                raise ValueError("exponential decay needs --init_learning_rate > 0")
+            lr_schedule = LRSchedule.exponential(int(steps_per_epoch * args.num_epochs_per_decay), args.learning_rate_decay_factor,
+                                                 floor=args.minimum_learning_rate / args.init_learning_rate, warmup_steps=warmup)
+        elif warmup:
+            lr_schedule = LRSchedule.constant(warmup_steps=warmup)
+    except ValueError as e:
+        raise SystemExit(f"tf_cnn_benchmarks (b200): learning-rate schedule: {e}")
     model = build_model(args.model, **({"image_size": S} if args.model == "trivial" else {}))
     loss_fn = nn.CrossEntropyLoss()
     dtype = torch.bfloat16 if on_gpu and (args.b200_compute_dtype == "bf16" or str(args.use_fp16).lower() == "true") else None
@@ -97,6 +132,7 @@ def main():
         print(f"Devices:     {['horovod/%s:%d' % (args.device, i) for i in range(size)]}")
         print(f"Data format: {args.data_format}")
         print(f"Optimizer:   {args.optimizer}")
+        print(f"LR:          {lr:g}" + (f" x {lr_schedule!r}" if lr_schedule is not None else ""))
         print(f"Variables:   {args.variable_update}")
         print(f"Engine:      {args.b200_engine} (NVLS multicast: {getattr(hvd._comm(), 'has_multicast', False)})")
         print("==========")
@@ -110,15 +146,16 @@ def main():
         trainer = DataParallelTrainer(model, loss_fn, hvd._comm(), lr=lr, momentum=mu, weight_decay=args.weight_decay,
                                       autocast_dtype=dtype, comm_backend="nccl" if args.b200_engine == "nccl" else "b200mpi",
                                       fused_optimizer=on_gpu, cuda_graph=on_gpu,
-                                      ema_decay=args.moving_average_decay if averaging else None)
+                                      ema_decay=args.moving_average_decay if averaging else None, lr_schedule=lr_schedule)
 
         def step():
             return trainer.step(x, y)
     else:
         dev = "cuda" if on_gpu else "cpu"
         model = model.to(dev).to(memory_format=torch.channels_last)
-        opt = torch.optim.SGD(model.parameters(), lr=lr, momentum=mu, weight_decay=args.weight_decay)
-        opt = hvd.DistributedOptimizer(opt, named_parameters=model.named_parameters(), op=hvd.Average)
+        sgd = torch.optim.SGD(model.parameters(), lr=lr, momentum=mu, weight_decay=args.weight_decay)
+        opt = hvd.DistributedOptimizer(sgd, named_parameters=model.named_parameters(), op=hvd.Average)
+        lr_sched = None   # a LambdaLR over the same multiplier, made once the resumed step count is known
         hvd.broadcast_parameters(model.state_dict(), root_rank=0)
         sx = torch.empty(B, 3, S, S, device=dev).contiguous(memory_format=torch.channels_last)
         sy = torch.empty(B, dtype=torch.long, device=dev)
@@ -131,10 +168,13 @@ def main():
                 loss = loss_fn(model(sx), sy)
             loss.backward()
             opt.step()
+            if lr_sched is not None:
+                lr_sched.step()
             return loss.detach()
 
     # --train_dir: resume / checkpoint (rank-0-only writer, the reference examples' convention: tensorflow_mnist.py:159)
     ckpt = os.path.join(args.train_dir, "model.ckpt.pt") if args.train_dir else ""
+    sched_step = 0   # the Horovod-API engine's schedule step count (the trainer keeps its own)
     if ckpt and os.path.exists(ckpt):
         sd = torch.load(ckpt, map_location="cpu", weights_only=False)
         # either engine reads what the other wrote: a trainer checkpoint carries masters / momentum / buffers by name, the
@@ -146,15 +186,23 @@ def main():
                 names = {n for n, _ in model.named_parameters()}
                 trainer.load_state_dict({"format": "b200mpi.DataParallelTrainer/1", "momentum": {},
                                          "model": {k: v for k, v in sd["model"].items() if k in names},
-                                         "buffers": {k: v for k, v in sd["model"].items() if k not in names}}, load_hyper=False)
+                                         "buffers": {k: v for k, v in sd["model"].items() if k not in names},
+                                         "lr_schedule_step": sd.get("lr_schedule_step", 0)}, load_hyper=False)
         elif "trainer" in sd:
             model.load_state_dict({**sd["trainer"]["model"], **sd["trainer"]["buffers"]})
+            sched_step = sd["trainer"].get("lr_schedule_step", 0)
         else:
             model.load_state_dict(sd["model"])
             opt.load_state_dict(sd["optimizer"])
+            sched_step = sd.get("lr_schedule_step", 0)
         if rank == 0:
             print(f"Restored checkpoint from {ckpt} (written after {sd.get('batches', '?')} batches on {sd.get('world', '?')} ranks)")
             sys.stdout.flush()
+
+    if lr_schedule is not None and args.b200_engine not in ("fused", "nccl"):
+        for g in sgd.param_groups:   # the base rate, whatever rate the loaded optimizer state was at
+            g["lr"] = g["initial_lr"] = lr
+        lr_sched = torch.optim.lr_scheduler.LambdaLR(sgd, lambda e: lr_schedule.multiplier(sched_step + e))
 
     def save_checkpoint(batches_done):
         if not ckpt:
@@ -163,6 +211,8 @@ def main():
             payload = {"trainer": trainer.state_dict()}          # collective: momentum shards are gathered
         else:
             payload = {"model": model.state_dict(), "optimizer": opt.state_dict()}
+            if lr_sched is not None:
+                payload["lr_schedule_step"] = sched_step + lr_sched.last_epoch
         if rank == 0:
             os.makedirs(args.train_dir, exist_ok=True)
             payload.update(batches=batches_done, world=size)

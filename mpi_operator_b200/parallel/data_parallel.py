@@ -32,6 +32,7 @@ import torch.nn as nn
 from ..ops import fused_bn
 from ..runtime.comm import Communicator, Window
 from ..utils import fault, nvtx
+from .lr_schedule import LRSchedule
 
 
 def _align(n: int, a: int) -> int:
@@ -308,6 +309,16 @@ class DataParallelTrainer:
         ...
         with trainer.ema_weights():            # collective when world > 1
             print(trainer.evaluate(x, y))
+
+    ``lr_schedule=LRSchedule...`` (``mpi_operator_b200.parallel.lr_schedule``) makes each group's learning rate
+    ``fp32(base * m(k))``, ``base`` the group's ``lr`` and ``k`` the number of synchronising steps before this one (the
+    CUDA-graph capture's warm-up steps included, ``no_sync()`` steps not). One single-CTA kernel on the compute stream
+    writes the rates into the device tables before each synchronising backward, so captured replays follow the schedule.
+    ``set_lr`` then sets the base rate, ``param_groups`` and checkpoints report base rates and ``current_lrs()`` the rates
+    of the last step. MLPerf's LARS recipe, linear warm-up then quadratic decay::
+
+        sched = LRSchedule.polynomial(total_steps=steps, power=2, warmup_steps=warmup)
+        trainer = DataParallelTrainer(model, loss_fn, comm, lr=peak_lr, lars=True, lr_schedule=sched, ...)
     """
 
     def __init__(self, model: nn.Module, loss_fn: Callable, comm: Communicator, *, lr: float, momentum: float = 0.9,
@@ -316,7 +327,9 @@ class DataParallelTrainer:
                  cuda_graph: bool = True, fused_optimizer: bool = True, algo: Optional[str] = None,
                  comm_backend: str = "b200mpi", bf16_params: Optional[bool] = None, async_h2d: Optional[bool] = None,
                  param_groups: Optional[list] = None, lars: bool = False, trust_coefficient: float = 0.001,
-                 ema_decay: Optional[float] = None):
+                 ema_decay: Optional[float] = None, lr_schedule: Optional[LRSchedule] = None):
+        if lr_schedule is not None and not isinstance(lr_schedule, LRSchedule):
+            raise ValueError(f"lr_schedule must be None or an LRSchedule, got {lr_schedule!r}")
         if ema_decay is not None and not (isinstance(ema_decay, (int, float)) and not isinstance(ema_decay, bool)
                                           and 0.0 < float(ema_decay) < 1.0):
             raise ValueError(f"ema_decay must be None or a number in (0, 1), got {ema_decay!r}")
@@ -368,6 +381,13 @@ class DataParallelTrainer:
         self._lr, self._mu, self._wd = lr, momentum, weight_decay
         # with param_groups: one {lr, momentum, weight_decay} row per group on the device, read by the kernels the same way
         self.group_hyper = torch.tensor(values, device=self.device, dtype=torch.float32) if self._tabled else None
+        # learning-rate schedule: the table, each group's base rate (float64) and the step count k on the device; the
+        # kernel rewrites the lr column of hyper / group_hyper from them every synchronising step
+        self.lr_schedule = lr_schedule
+        if lr_schedule is not None:
+            self._lr_table = torch.tensor(lr_schedule.table(), dtype=torch.float64, device=self.device)
+            self._lr_base = torch.tensor([float(v[0]) for v in values], dtype=torch.float64, device=self.device)
+            self._lr_step = torch.zeros(1, dtype=torch.int64, device=self.device)
         self._lars_board = self._lars_scratch = None
         if self._lars:
             self._alloc_lars()
@@ -429,9 +449,17 @@ class DataParallelTrainer:
     # ---------------------------------------------------------- hyper --
     def set_lr(self, lr: float, group: Optional[int] = None) -> None:
         """Learning rate of every group (``group=None``) or of group ``group`` (an index into ``param_groups``; group 0
-        holds the trainer-level values). Takes effect from the next step, CUDA-graph replays included."""
+        holds the trainer-level values). Takes effect from the next step, CUDA-graph replays included. With ``lr_schedule``
+        it sets the base rate the schedule multiplies."""
         if group is not None and not 0 <= group < len(self._group_vals):
             raise IndexError(f"group {group} out of range: the trainer has {len(self._group_vals)} parameter groups")
+        if self.lr_schedule is not None:
+            if group is None or group == 0:
+                self._lr = lr
+            for k in (range(len(self._group_vals)) if group is None else (group,)):
+                self._group_vals[k][0] = lr
+                self._lr_base[k] = float(lr)
+            return
         if group is None or group == 0:
             self._lr = lr
             self.hyper[0] = lr
@@ -442,6 +470,36 @@ class DataParallelTrainer:
                 self.group_hyper[:, 0] = lr
             else:
                 self.group_hyper[group, 0] = lr
+
+    def _schedule_step(self) -> None:
+        """Write the scheduled rates of step k into the lr column of the tables and advance k."""
+        sch = self.lr_schedule
+        if self._cuda:
+            self.comm.lr_schedule(self._lr_table, sch.form, len(sch.boundaries), self._lr_step, self._lr_base, self.hyper,
+                                  self.group_hyper, stream=torch.cuda.current_stream(self.device))
+            return
+        k = int(self._lr_step)
+        self._write_rates(k)
+        self._lr_step += 1
+
+    def _write_rates(self, k: int) -> None:
+        """The rates of step ``k`` (``LRSchedule.rate``: the kernel's bits) into the lr column of the tables."""
+        rates = [self.lr_schedule.rate(v[0], k) for v in self._group_vals]
+        self.hyper[0] = rates[0]
+        if self.group_hyper is not None:
+            self.group_hyper[:, 0] = torch.tensor(rates, dtype=torch.float32)
+
+    def current_lrs(self) -> list:
+        """Each group's learning rate as the last synchronising step used it (with a schedule: the base rates before the
+        first step). Reading it synchronises with the device."""
+        if self.group_hyper is not None:
+            return [float(v) for v in self.group_hyper[:, 0].tolist()]
+        return [float(self.hyper[0])]
+
+    @property
+    def lr_schedule_step(self) -> int:
+        """k: the synchronising steps the schedule has seen (reading it synchronises with the device)."""
+        return int(self._lr_step) if self.lr_schedule is not None else 0
 
     @property
     def param_groups(self) -> list:
@@ -648,6 +706,8 @@ class DataParallelTrainer:
             torch._foreach_add_(counters, 1)
         if self._sync and self._ema_sched is not None:   # k of this update; the bucket kernels read it after the main->comm event
             self._ema_sched[1:].add_(1)
+        if self._sync and self.lr_schedule is not None:  # this update's rates, read the same way
+            self._schedule_step()
         with nvtx.range("b200mpi.backward+allreduce_sgd"):   # bucket kernels are launched from the autograd hooks inside
             loss.backward()
         self._loss.copy_(loss.detach())
@@ -878,7 +938,7 @@ class DataParallelTrainer:
             momentum[names[p]] = mom_flat[start:start + n].as_strided(p.size(), p.stride()).detach().cpu().contiguous()
         sd = {"format": "b200mpi.DataParallelTrainer/1", "model": masters, "momentum": momentum,
               "buffers": {n: b.detach().cpu().clone() for n, b in self.model.named_buffers()},
-              "hyper": {"lr": float(self.hyper[0]), "momentum": float(self.hyper[1]), "weight_decay": float(self.hyper[2]),
+              "hyper": {"lr": float(self.hyper[0]) if self.lr_schedule is None else float(self._lr), "momentum": float(self.hyper[1]), "weight_decay": float(self.hyper[2]),
                         "nesterov": bool(self.nesterov), "lars": bool(self._group_lars[0]),
                         "trust_coefficient": self.trust_coefficient},
               "world_size_at_save": int(self.comm.world)}
@@ -890,6 +950,9 @@ class DataParallelTrainer:
                          .detach().cpu().contiguous() for p in st.params}
             sd["ema_updates"] = self.ema_updates
             sd["hyper"]["ema_decay"] = self.ema_decay
+        if self.lr_schedule is not None:
+            sd["lr_schedule"] = self.lr_schedule.to_dict()
+            sd["lr_schedule_step"] = self.lr_schedule_step
         return sd
 
     def _gather_shards(self, attr: str) -> torch.Tensor:
@@ -973,7 +1036,8 @@ class DataParallelTrainer:
         momentum is the same state for SGD and LARS, so SGD and LARS checkpoints load into each other. With ``ema_decay`` the
         weight average and its update count are restored from ``"ema"`` / ``"ema_updates"``, or, for a checkpoint without
         them, restart from the loaded parameters at count 0; the decay stays this trainer's. Without ``ema_decay`` they are
-        ignored."""
+        ignored. With ``lr_schedule`` the step count comes back from ``"lr_schedule_step"`` (0 when absent), the loaded
+        ``lr`` values are the base rates and the schedule stays this trainer's; without it both keys are ignored."""
         if self._in_ema:
             raise RuntimeError("load_state_dict() inside ema_weights(): leaving the context would undo it")
         if sd.get("format") != "b200mpi.DataParallelTrainer/1":
@@ -1034,6 +1098,14 @@ class DataParallelTrainer:
             if self._has_groups:
                 self._group_vals = [[g["lr"], g["momentum"], g["weight_decay"]] for g in sd["param_groups"]]
                 self.group_hyper.copy_(torch.tensor(self._group_vals, dtype=torch.float32))
+        if self.lr_schedule is not None:
+            k = int(sd.get("lr_schedule_step", 0))
+            if k < 0:
+                raise ValueError(f"lr_schedule_step must be >= 0, got {k}")
+            self._lr_base.copy_(torch.tensor([float(v[0]) for v in self._group_vals], dtype=torch.float64))
+            self._lr_step.fill_(k)
+            if k > 0:   # the tables hold what the last step used, as after that step
+                self._write_rates(k - 1)
         if self._cuda:
             torch.cuda.synchronize(self.device)
 

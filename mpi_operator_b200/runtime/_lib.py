@@ -91,6 +91,7 @@ def lib() -> C.CDLL:
     L.b200mpi_slice_elems.argtypes = [sz, i, i]
     L.b200mpi_slice_elems.restype = sz
     L.b200mpi_set_hyper_ptr.argtypes = [vp, vp]
+    L.b200mpi_lr_schedule.argtypes = [vp, vp, i, i, vp, vp, i, vp, vp, vp]
     L.b200mpi_broadcast.argtypes = [vp, vp, sz, i, i, vp]
     L.b200mpi_broadcast_bytes.argtypes = [vp, vp, sz, i, vp]
     L.b200mpi_allgather.argtypes = [vp, vp, vp, sz, i, vp]

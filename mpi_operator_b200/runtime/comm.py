@@ -495,6 +495,34 @@ class Communicator:
         self._hyper = tensor
         check(_lib.lib().b200mpi_set_hyper_ptr(self._h, tensor.data_ptr() if tensor is not None else None))
 
+    def lr_schedule(self, table, form: int, num_boundaries: int, step, base, hyper, group_hyper=None, stream=None) -> None:
+        """One launch of ``k_lr_schedule`` on ``stream``; see b200mpi_lr_schedule. ``table`` is the float64 table of
+        ``LRSchedule.table()`` on the device, ``step`` an int64 counter of one element, ``base`` the float64 base rates
+        ``[G]``, ``hyper`` the ``set_hyper`` tensor and ``group_hyper`` the optional float32 ``[G, 3]`` group table; all
+        contiguous CUDA tensors on this communicator's device. Writes the rates of step ``step`` and advances it by one."""
+        torch = _torch()
+        dev = torch.device("cuda", self.device)
+
+        def ok(t, dtype, n=None):
+            return t.device == dev and t.dtype == dtype and t.is_contiguous() and (n is None or t.numel() == n)
+        if not ok(table, torch.float64):
+            raise B200MPIError(f"lr_schedule: table must be a contiguous float64 tensor on {dev}")
+        if not ok(step, torch.int64, 1):
+            raise B200MPIError(f"lr_schedule: step must be a contiguous int64 tensor of 1 element on {dev}")
+        if not (ok(base, torch.float64) and base.dim() == 1 and 1 <= base.numel() <= 256):
+            raise B200MPIError(f"lr_schedule: base must be a contiguous float64 [G] tensor on {dev}, 1 <= G <= 256")
+        G = base.numel()
+        if not (ok(hyper, torch.float32) and hyper.numel() >= 1):
+            raise B200MPIError(f"lr_schedule: hyper must be a contiguous float32 tensor on {dev}")
+        if group_hyper is not None and not (ok(group_hyper, torch.float32, 3 * G) and group_hyper.dim() == 2):
+            raise B200MPIError(f"lr_schedule: group_hyper must be a contiguous float32 [{G}, 3] tensor on {dev}")
+        if table.numel() < 1 + (2 * num_boundaries + 1 if form == 1 else 3 if form in (2, 3) else 0):
+            raise B200MPIError("lr_schedule: table shorter than its form and boundary count need")
+        check(_lib.lib().b200mpi_lr_schedule(self._h, table.data_ptr(), int(form), int(num_boundaries), step.data_ptr(),
+                                             base.data_ptr(), G, hyper.data_ptr(),
+                                             group_hyper.data_ptr() if group_hyper is not None else None,
+                                             _stream_ptr(stream)), "lr_schedule")
+
     def slice_elems(self, count: int, dtype) -> int:
         return int(_lib.lib().b200mpi_slice_elems(count, self.world, dtype_code(dtype)))
 
