@@ -214,7 +214,7 @@ k_bn_fwd_finalize(const __nv_bfloat16* __restrict__ x, const float* __restrict__
   const float d = S1 * inv_m;
   const float mean = k + d;
   float var = fmaf(-d, d, S2 * inv_m);
-  var = var > 0.f ? var : 0.f;
+  var = var < 0.f ? 0.f : var;   // rounding can leave a tiny negative variance; NaN passes, as in PyTorch
   const float invstd = rsqrtf(var + eps);
   save_mean[c] = mean;
   save_invstd[c] = invstd;
@@ -264,9 +264,9 @@ k_bn_fwd_apply(const uint4* __restrict__ x, const uint4* __restrict__ res, uint4
         for (int j = 0; j < 8; j++) {
           float z = fmaf(a[j], f[j], b[j]);
           if (RES) z += g[j];
-          if (RELU) {
-            bits |= (z > 0.f ? 1u : 0u) << j;
-            z = z > 0.f ? z : 0.f;
+          if (RELU) {   // as torch.relu / threshold_backward: NaN passes, with its gradient
+            bits |= (z <= 0.f ? 0u : 1u) << j;
+            z = z <= 0.f ? 0.f : z;
           }
           f[j] = z;
         }
@@ -318,7 +318,7 @@ k_bn_eval_apply(const uint4* __restrict__ x, const uint4* __restrict__ res, uint
         for (int j = 0; j < 8; j++) {
           float z = fmaf(a[j], f[j], b[j]);
           if (RES) z += g[j];
-          if (RELU) z = z > 0.f ? z : 0.f;
+          if (RELU) z = z <= 0.f ? 0.f : z;
           f[j] = z;
         }
         stg_stream(y + mm * tpr + cg, pack8(f));
@@ -442,6 +442,11 @@ k_bn_bwd_elemt(const uint4* __restrict__ dz, const uint4* __restrict__ x, const 
   }
 }
 
+// Every activation is read and written as 16-byte vectors (null pointers pass: optional operands).
+static bool aligned16(const void* a, const void* b = nullptr, const void* c = nullptr) {
+  return (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15) == 0;
+}
+
 static long long env_chunk(const char* name, long long dflt) {
   const char* v = getenv(name);
   return v && *v ? atoll(v) : dflt;
@@ -481,6 +486,7 @@ int b200mpi_bn_act_fwd(const void* x, const void* residual, void* y, void* mask,
                        float* running_mean, float* running_var, float* save_mean, float* save_invstd, float* workspace,
                        long long M, int C, float eps, float momentum, int relu, void* stream_) {
   if (!b200mpi_bn_supported(M, C)) return B200MPI_ERR_UNSUPPORTED;
+  if (!aligned16(x, residual, y)) return B200MPI_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream_;
   float* coef = workspace;
   float* partials = workspace + 4 * C;
@@ -508,6 +514,7 @@ int b200mpi_bn_act_fwd_prestats(const void* x, const void* residual, void* y, vo
   if (!b200mpi_bn_supported(M, C) || parts < 1 || !partials || M >= (1LL << 31) - b200mpi::gemm::BM ||
       (long long)(parts - 1) * b200mpi::gemm::BM >= M)
     return B200MPI_ERR_UNSUPPORTED;
+  if (!aligned16(x, residual, y)) return B200MPI_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream_;
   float* coef = workspace;
   int grid;
@@ -559,6 +566,7 @@ int b200mpi_bn_act_bwd_prestats(const void* dz, const void* x, const void* mask,
                                 const float* save_mean, const float* save_invstd, float* dweight, float* dbias, float* workspace,
                                 const float* partials, int parts, long long M, int C, int relu, void* stream_) {
   if (!b200mpi_bn_supported(M, C) || parts < 1 || !partials) return B200MPI_ERR_UNSUPPORTED;
+  if (!aligned16(dz, x, dx) || !aligned16(dres)) return B200MPI_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream_;
   float* coef = workspace;
   k_bn_bwd_finalize<<<(2 * C + kMergeOut - 1) / kMergeOut, kThreadsBN, 0, s>>>(partials, parts, coef, M, C, weight, save_mean, save_invstd, dweight, dbias);
@@ -570,6 +578,7 @@ int b200mpi_bn_act_bwd(const void* dz, const void* x, const void* mask, void* dx
                        const float* save_mean, const float* save_invstd, float* dweight, float* dbias, float* workspace,
                        long long M, int C, int relu, void* stream_) {
   if (!b200mpi_bn_supported(M, C)) return B200MPI_ERR_UNSUPPORTED;
+  if (!aligned16(dz, x, dx) || !aligned16(dres)) return B200MPI_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream_;
   float* coef = workspace;
   float* partials = workspace + 4 * C;

@@ -326,9 +326,9 @@ k_gemm_bnstats(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
             v0 += __uint_as_float(r2 << 16);
             v1 += __uint_as_float(r2 & 0xffff0000u);
           }
-          if (relu) {
-            v0 = v0 > 0.f ? v0 : 0.f;
-            v1 = v1 > 0.f ? v1 : 0.f;
+          if (relu) {   // as torch.relu: NaN passes
+            v0 = v0 <= 0.f ? 0.f : v0;
+            v1 = v1 <= 0.f ? 0.f : v1;
           }
           d[4 * j + 2 * i] = v0;
           d[4 * j + 2 * i + 1] = v1;

@@ -33,7 +33,9 @@ def fused_bn_available(x: torch.Tensor, bn: torch.nn.BatchNorm2d) -> bool:
     # one value per channel: training-mode batch norm is undefined, and nn.BatchNorm2d's error should reach the caller
     if n * h * w < 2:
         return False
-    return bool(_lib().b200mpi_bn_supported(n * h * w, c)) and x.is_contiguous(memory_format=torch.channels_last)
+    # the kernels move 16-byte vectors: a view at an odd storage offset takes the PyTorch path
+    return (bool(_lib().b200mpi_bn_supported(n * h * w, c)) and x.is_contiguous(memory_format=torch.channels_last)
+            and x.data_ptr() % 16 == 0)
 
 
 def _eval_bn_ready(bn: torch.nn.BatchNorm2d, *inputs) -> bool:
@@ -162,6 +164,8 @@ class _BNAct(torch.autograd.Function):
         m = n * h * w
         if dz.dtype != torch.bfloat16 or not dz.is_contiguous(memory_format=torch.channels_last):
             dz = dz.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+        if dz.data_ptr() % 16:
+            dz = dz.clone(memory_format=torch.channels_last)
         dx = torch.empty_like(x, memory_format=torch.channels_last)
         dres = torch.empty_like(x, memory_format=torch.channels_last) if ctx.has_res else None
         direct = (ctx.direct is not None and ctx.wb[0].grad is not None and ctx.wb[1].grad is not None
@@ -195,11 +199,11 @@ def bn_act(bn: torch.nn.BatchNorm2d, x: torch.Tensor, residual: torch.Tensor = N
         if residual is None or residual.data_ptr() % 16 == 0:
             return _bn_eval(bn, x, residual, relu)
     if fused_bn_available(x, bn) and (residual is None or (residual.dtype == torch.bfloat16 and residual.shape == x.shape)):
-        if residual is not None and not residual.is_contiguous(memory_format=torch.channels_last):
-            residual = residual.contiguous(memory_format=torch.channels_last)
-        _count_batch(bn)
-        return _BNAct.apply(x, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, _ws(bn, x.device), bn.eps,
-                            bn.momentum, relu, getattr(bn, "_b200_grad_ready", None))
+        residual = _residual_cl(residual)
+        if residual is None or residual.data_ptr() % 16 == 0:
+            _count_batch(bn)
+            return _BNAct.apply(x, residual, bn.weight, bn.bias, bn.running_mean, bn.running_var, _ws(bn, x.device), bn.eps,
+                                bn.momentum, relu, getattr(bn, "_b200_grad_ready", None))
     out = bn(x)
     if residual is not None:
         out = out + residual
@@ -308,6 +312,8 @@ class _Conv1x1BNAct(torch.autograd.Function):
             ctx.handed.partials = None
         if dz.dtype != torch.bfloat16 or not dz.is_contiguous(memory_format=torch.channels_last):
             dz = dz.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+        if dz.data_ptr() % 16:
+            dz = dz.clone(memory_format=torch.channels_last)
         dy = torch.empty(m, cout, dtype=torch.bfloat16, device=dz.device)          # gradient w.r.t. the convolution output
         accumulating = ctx.direct is not None and getattr(ctx.direct, "accumulating", _never)()
         # residual side of a link: the residual gradient mask ⊙ dz goes to conv1's dgrad epilogue, not to autograd

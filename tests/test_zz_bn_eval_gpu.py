@@ -2,7 +2,9 @@
 ``b200mpi_gemm_bn_eval``, their dispatch from ``bn_act`` / ``conv_bn_act``, whole ResNets in eval mode, and
 ``DataParallelTrainer.evaluate()`` under a CUDA graph.
 
-References are float64 computations on the same bf16 operands. BatchNorm layers get random gamma / beta and running
+References are float64 computations on the same bf16 operands, and the oracle of tests/bn_oracle.py: rsqrtf is not
+correctly rounded, so per channel one of the fp32 values within 2 ulps of the correctly rounded rsqrt must reproduce the
+kernel's whole column bit for bit. BatchNorm layers get random gamma / beta and running
 statistics (mean ~ N(0, 1), var ~ U(0.1, 4)): ResNet zero-initialises bn3.weight, which would hide every error on the residual
 branch. Each case runs in a subprocess, so that a trap in a kernel cannot poison the CUDA context of the test session."""
 import os
@@ -16,8 +18,10 @@ pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 PRELUDE = r"""
-import os, sys, copy, ctypes, torch, torch.nn as nn
+import os, sys, copy, ctypes, numpy as np, torch, torch.nn as nn
 sys.path.insert(0, {repo!r})
+sys.path.insert(0, os.path.join({repo!r}, "tests"))
+import bn_oracle as O
 from mpi_operator_b200.ops import fused_bn, gemm_bnstats
 torch.manual_seed(0)
 dev = torch.device("cuda")
@@ -46,6 +50,15 @@ def coef_mag64(bn):
     a, _ = coef64(bn)
     m = (bn.running_mean.double() * a).abs()
     return m + bn.bias.double().abs() if bn.bias is not None else m
+
+def exact_columns(y, x, r, bn, relu, what):
+    # rows [0, 2048) and the last 256: the eval kernels have no reduction, every row is computed alike
+    M = x.shape[0]
+    idx = torch.tensor(sorted(set(range(min(M, 2048))) | set(range(max(0, M - 256), M))), device=x.device)
+    found = O.eval_match(O._bits(y[idx]), O.to_np(x[idx]), None if r is None else O.to_np(r[idx]), O.to_np(bn.weight),
+                         O.to_np(bn.bias), O.to_np(bn.running_mean), O.to_np(bn.running_var), bn.eps, relu)
+    bad = np.nonzero(np.abs(found) > 2)[0]
+    assert bad.size == 0, (what, "no rsqrtf candidate reproduces channels", bad[:8].tolist())
 
 def ulp(ref):
     # one bf16 ulp at |ref| (8 significant bits)
@@ -103,6 +116,8 @@ for M in (1, 7, 1000, 200704):
                     assert bool((got >= 0).all())
                     neg = t < -1e-6 * mag
                     assert bool((got[neg] == 0).all()), ("zeros", C, M, use_res)
+            exact_columns(z.reshape(M, C), x.reshape(M, C), r.reshape(M, C) if use_res else None, bn, relu,
+                          ("kernel", C, M, use_res, relu))
 for a, b in zip(bufs, (bn.running_mean, bn.running_var, bn.num_batches_tracked)):
     assert torch.equal(a, b), "running statistics changed"
 assert all(torch.equal(ws[k], fused_bn._WS_CACHE[k]) for k in ws) and set(ws) == set(fused_bn._WS_CACHE), "workspace changed"
@@ -168,6 +183,35 @@ print("OK")
 @pytest.mark.parametrize("m,k,n", GEMM_SHAPES)
 def test_gemm_bn_eval_epilogue_matches_fp64(m, k, n):
     _run(GEMM_CASE, m=m, k=k, n=n)
+
+
+# The epilogue on gemm_oracle's family E: the fp32 accumulator is exact, so a * acc + b (+ r) is checked bit for bit with the
+# candidate rsqrtf; tile widths 128 and 64 (N = 192), and a full ResNet-101 layer.
+GEMM_EXACT_CASE = r"""
+import gemm_oracle as G
+M, K, N = {m}, {k}, {n}
+op = G.family_e(M, N, K, x_full=True, seed=M + N, device="cuda")
+acc, mag = G.ref_chunk(op, 0, M)
+G.check_exact_precondition(op, 0, M, mag)
+acc32 = acc.float()
+assert torch.equal(acc32.double(), acc)
+bn = nn.BatchNorm2d(N).cuda().eval()
+randomize_bn(bn)
+with torch.no_grad():
+    bn.running_mean.mul_(acc.abs().mean())              # the conv output's scale: b matters against a * acc
+    bn.running_var.mul_(acc.var(0).mean())
+r = torch.randn(M, N, device=dev).to(torch.bfloat16)
+for use_res in (False, True):
+    for relu in (False, True):
+        y = gemm_bnstats.gemm_bn_eval(op.x, op.w, bn, r if use_res else None, relu)
+        exact_columns(y, acc32, r if use_res else None, bn, relu, ("gemm", M, K, N, use_res, relu))
+print("OK")
+"""
+
+
+@pytest.mark.parametrize("m,k,n", [(1000, 64, 128), (1000, 64, 192), (64 * 7 * 7, 512, 2048)])
+def test_gemm_bn_eval_epilogue_exact_on_exact_accumulators(m, k, n):
+    _run(GEMM_EXACT_CASE, m=m, k=k, n=n)
 
 
 # ------------------------------------------------------------------------------------------------------- dispatch --

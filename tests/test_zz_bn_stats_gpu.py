@@ -1,7 +1,9 @@
 """BatchNorm statistics of the fused kernels against float64, at the shapes ResNet-101 runs at batch 64.
 
 The reference is float64 PyTorch on the same bf16-rounded inputs the kernels read. fp32 outputs (save_mean, save_invstd,
-running stats, dgamma, dbeta) are compared directly, bf16 outputs elementwise. Covered:
+running stats, dgamma, dbeta) are compared directly, bf16 outputs elementwise. The bn_act.cu cases are also held bit for bit
+to the oracle of tests/bn_oracle.py (the float64 bounds say the algorithm is accurate, the oracle that it is the one the
+kernels implement), and each of ResNet-101's layers has at least one output that is an exact bf16 tie. Covered:
   * bn_act.cu through its C entry points (forward + backward, with and without residual and ReLU) at ResNet-101's (M, C)
     pairs, at every supported channel count, and with the reduce grid forced to its 296-row cap and to a single CTA;
   * the fused 1x1 path (conv_bn_act -> gemm_bnstats_shifted -> b200mpi_bn_act_fwd_prestats) on conv outputs with
@@ -28,23 +30,14 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 skip_gemm = pytest.mark.skipif(os.environ.get("B200MPI_SKIP_GEMM_TESTS") == "1", reason="B200MPI_SKIP_GEMM_TESTS=1")
 
 EPS, MOMENTUM = 1e-5, 0.1
-THREADS, UNROLL, MAX_PARTS = 256, 4, 296   # bn_act.cu: kThreadsBN, kUnroll, kMaxParts
-REDUCE_CHUNK = 64 << 10                    # bn_act.cu: default of B200MPI_BN_REDUCE_CHUNK
+from bn_oracle import MAX_PARTS, REDUCE_CHUNK, THREADS, plan_rows  # noqa: E402
+import bn_oracle  # noqa: E402
+
 ULP_REL = 2.0 ** -7                        # one bf16 ulp, relative: the rounding of every bf16 output
 
 # (M = N*H*W, C) of ResNet-101's BatchNorm layers at batch 64 (224x224 input)
 RESNET101 = [(802816, 64), (200704, 64), (200704, 128), (200704, 256), (50176, 128), (50176, 512), (12544, 256),
              (12544, 1024), (3136, 512), (3136, 2048)]
-
-
-def plan_rows(m, c, bytes_per_row, chunk=REDUCE_CHUNK):
-    """Partial rows a reduce-type kernel of bn_act.cu writes (its plan(): >= `chunk` bytes and >= 4 row passes per CTA,
-    at most MAX_PARTS CTAs, rows per CTA rounded up to whole passes). Forward stats read 2C bytes per row, backward 4C."""
-    rpp = THREADS // (c // 8)
-    g = max(1, min((m + rpp * UNROLL - 1) // (rpp * UNROLL), (m * bytes_per_row + chunk - 1) // chunk, MAX_PARTS))
-    rows = (m + g - 1) // g
-    rows = (rows + rpp - 1) // rpp * rpp
-    return (m + rows - 1) // rows
 
 
 # ------------------------------------------------------------------------------------------------ helpers ----
@@ -181,8 +174,9 @@ def make_bn_inputs(m, c, use_res, seed):
 
 # ------------------------------------------------------------------------------------------- bn_act.cu ----
 def check_bn_act(m, c, relu, use_res, chunk=REDUCE_CHUNK, calls=3):
-    """Forward `calls` times and backward twice on the same inputs; everything against float64, and every repeat bitwise
-    equal to the first. Returns the partial-row counts of the forward and backward reduce grids."""
+    """Forward `calls` times and backward twice on the same inputs; everything against float64 and bit for bit against
+    the oracle (tests/bn_oracle.py), and every repeat bitwise equal to the first. Returns the partial-row counts of the
+    forward and backward reduce grids and the bf16 ties among y and dx."""
     x, res, gamma, beta, dz = make_bn_inputs(m, c, use_res, seed=m + c)
     rm = torch.zeros(c, device="cuda")
     rv = torch.ones(c, device="cuda")
@@ -195,13 +189,21 @@ def check_bn_act(m, c, relu, use_res, chunk=REDUCE_CHUNK, calls=3):
     fwd_rows = rows_written(ws, c)
     assert fwd_rows == plan_rows(m, c, 2 * c, chunk), (tag, fwd_rows)
     assert_running(rm, rv, *ref_running(rm0, rv0, mu, var, m, 1), tag + " after 1 call")
+    y, mask, mean, invstd = first
+    fin, y_ties = bn_oracle.check_forward(x, res, y, mask, mean, invstd, ws, gamma, beta, rm0, rv0, rm, rv, EPS, MOMENTUM, relu,
+                                          chunk=chunk, what=tag)
+    want_rm, want_rv = fin["rm"], fin["rv"]
     for _ in range(calls - 1):
         again = bn_fwd(x, res, gamma, beta, rm, rv, relu, ws)
         for a, b in zip(first, again):
             assert a is None or torch.equal(a, b), tag + ": forward not deterministic"
+        fin = bn_oracle.fwd_finalize(bn_oracle.merge(bn_oracle.to_np(ws[4 * c:4 * c + fwd_rows * 2 * c]).reshape(fwd_rows, -1)),
+                                     bn_oracle.to_np(x[0]), m, None, None, want_rm, want_rv, EPS, MOMENTUM, invstd=fin["invstd"])
+        want_rm, want_rv = fin["rm"], fin["rv"]
+    bn_oracle.assert_bits(rm, want_rm, tag + " running_mean after every call")
+    bn_oracle.assert_bits(rv, want_rv, tag + " running_var after every call")
     assert_running(rm, rv, *ref_running(rm0, rv0, mu, var, m, calls), tag + f" after {calls} calls")
 
-    y, mask, mean, invstd = first
     assert_stats(mean, invstd, mu, var, inv, tag)
     z = (xd - mu) * inv * gamma.double() + beta.double()
     if use_res:
@@ -220,18 +222,22 @@ def check_bn_act(m, c, relu, use_res, chunk=REDUCE_CHUNK, calls=3):
     for a, b in zip(grads, bn_bwd(dz, x, mask, gamma, mean, invstd, relu, use_res, ws)):
         assert a is None or torch.equal(a, b), tag + ": backward not deterministic"
     dx, dres, dgamma, dbeta = grads
+    dx_ties = bn_oracle.check_backward(dz, x, mask, dx, dres, dgamma, dbeta, ws, gamma, mean, invstd, relu, chunk=chunk, what=tag)
     g, ref_dx, ref_dgamma, ref_dbeta, abs_gx, abs_g = ref_bwd(dz, xd, bits if relu else None, gamma, mu, inv, relu)
     assert_param_grads(dgamma, dbeta, ref_dgamma, ref_dbeta, abs_gx, abs_g, tag)
     assert_elementwise(dx, ref_dx, tag + " dx")
     if use_res:
         assert_elementwise(dres, g, tag + " dres")
-    return fwd_rows, bwd_rows
+    print(f"{tag}: bf16 ties among y {y_ties}, among dx {dx_ties}")
+    return fwd_rows, bwd_rows, y_ties, dx_ties
 
 
 @pytest.mark.parametrize("relu,use_res", [(True, True), (True, False), (False, True), (False, False)])
 @pytest.mark.parametrize("m,c", RESNET101)
 def test_bn_act_resnet101_shapes_match_fp64(m, c, relu, use_res):
-    fwd_rows, bwd_rows = check_bn_act(m, c, relu, use_res)
+    fwd_rows, bwd_rows, y_ties, dx_ties = check_bn_act(m, c, relu, use_res)
+    # the oracle has decided round-to-nearest-even ties at every one of these shapes
+    assert y_ties + dx_ties > 0
     # every layer merges >= 97 partial rows in at least one direction: the merge's 4-way unrolled loop runs
     assert max(fwd_rows, bwd_rows) >= 97
     if (m, c) == (802816, 64):
@@ -286,13 +292,13 @@ def _run(expr, env=None, timeout=900):
 def test_bn_act_reduce_grid_at_its_cap_for_a_small_layer():
     # a 1-byte chunk leaves the CTA count to the row rule and the cap: 37888 rows at C = 64 give exactly 296 CTAs
     assert plan_rows(37888, 64, 2 * 64, chunk=1) == plan_rows(37888, 64, 4 * 64, chunk=1) == MAX_PARTS
-    _run("assert T.check_bn_act(37888, 64, True, True, chunk=1) == (T.MAX_PARTS, T.MAX_PARTS)",
+    _run("assert T.check_bn_act(37888, 64, True, True, chunk=1)[:2] == (T.MAX_PARTS, T.MAX_PARTS)",
          env={"B200MPI_BN_REDUCE_CHUNK": "1"})
 
 
 def test_bn_act_reduce_grid_of_one_cta():
     # one CTA over all of M: ~6,300 serial fp32 adds per thread at M = 200704, C = 64
-    _run("assert T.check_bn_act(200704, 64, True, False, chunk=10**15, calls=1) == (1, 1)",
+    _run("assert T.check_bn_act(200704, 64, True, False, chunk=10**15, calls=1)[:2] == (1, 1)",
          env={"B200MPI_BN_REDUCE_CHUNK": str(10 ** 15)})
 
 
